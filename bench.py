@@ -15,8 +15,8 @@ weights in the reference's checkpoint format, mem_freq 5):
 ONE STEP = the interaction(s) of the configuration on every clip a GPU holds: `--clips-per-gpu` concurrent
 lanes (own network object, CUDA stream, Python thread) x `--lockstep` clips per lane advanced as one
 batch (mivos_b200.LockstepSession).  The JSON line carries, measured in the same run:
-  value / e2e                    the headline configuration (fp16 operands; cfg2: 3 lanes x 4 lock-step clips; measured
-                                 on B200, profiles/r02c9_bench_c*_l4.json: 3 x 4 1060 frames/s, 2 x 4 1038)
+  value / e2e                    the headline configuration (fp16 operands; cfg2: 2 lanes x 4 lock-step clips, the
+                                 most 101-frame sessions whose TF32 companion run also fits the 80 GB of an H100)
                                  value: clips resident in HBM; e2e: clips in PINNED HOST memory, every frame
                                  copied H2D inside the timed region, u8 masks copied D2H at the end
   single_session                 the same metric through ONE InferenceCore.interact (1 lane x 1 clip): what
@@ -33,9 +33,12 @@ with the memory bank PRE-FILLED to the mean bank size a frame of the full clip s
 the per-frame cost of the reference is linear in the bank size, so the sample's frames cost what the
 average frame of the full clip costs) — same shapes, same top-k, same per-frame work as `config`.
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.
-Every step reads a whole clip (503 MB at cfg2) plus >200 MB of weights: inputs exceed the 126 MB L2.
+Every step reads a whole clip (503 MB at cfg2) plus >200 MB of weights: inputs exceed the 50 MB L2.
 Multi-GPU: clips shard across ranks (weak scaling, no data-path collective); NCCL only for the barrier
 and the max/sum reductions of the timings.
+--dump-outputs DIR: after the timed steps of the headline measurement, what its last step returned to the
+caller, per clip c: DIR/masks_c<c>.npy (the u8 masks of interact()) and DIR/prob_c<c>.npy (InferenceCore.prob),
+each a fixed seeded sample of at most 262144 elements as float32 (inputs are seeded: two builds compare output for output).
 """
 from __future__ import annotations
 
@@ -48,6 +51,7 @@ import sys
 import threading
 import time
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -61,7 +65,7 @@ ACT_DTYPE = torch.float32  # set from --act in main()
 # lanes / lockstep: clips a GPU propagates at a time in the headline measurement of each configuration;
 # ref_frames / ref_bank: the bounded CPU sample (frames of the sub-clip, pre-filled certain bank frames)
 CONFIGS = {
-    "cfg2": dict(H=480, W=854, K=1, top_k=20, frames=101, inter=(0,), lanes=3, lockstep=4, ref_frames=11, ref_bank=10,
+    "cfg2": dict(H=480, W=854, K=1, top_k=20, frames=101, inter=(0,), lanes=2, lockstep=4, ref_frames=11, ref_bank=10,
                  metric=METRIC, label="cfg2: DAVIS-shaped 480p (480x854 -> 480x864), 1 object, 101-frame clip, mem_freq 5, "
                                       "bank 1->21 frames, top-k 20"),
     "cfg3": dict(H=480, W=854, K=3, top_k=50, frames=251, inter=(0,), lanes=2, lockstep=1, ref_frames=4, ref_bank=25,
@@ -84,13 +88,13 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 — a bound, not a rate this card reached
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback (H100 SXM data sheet)"
 
 
 def _measured_traffic(fp16: bool):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, from THIS round's
-    `ncu --set full` capture (profiles/r02_traffic.json, written by tools/ncu_summary.py traffic); null when no
-    capture of the current kernels is committed."""
+    """DRAM bytes of one launch of the dominant kernel from a committed profiler capture
+    (profiles/r02_traffic.json); null when no capture of the current kernels is committed."""
     p = os.path.join(ROOT, "profiles", "r02_traffic.json")
     if not os.path.exists(p):
         return None, None
@@ -319,7 +323,7 @@ def _bracketed_pass(mivos_b200, ops, net, clips, masks, dev, fuse=None, inter=(0
     saved_env = os.environ.get("MIVOS_GRAPH")
     # the batched query pass normally runs on the network's side stream, concurrently with the frame loop: a
     # bracket around a launch of one stream would then include whatever the other stream's kernels took from it
-    # (r02c9: the same memory read bracketed at 457 us and at 885 us in two runs).  For this pass the query pass
+    # (the same memory read can then be bracketed at twice its time).  For this pass the query pass
     # is issued on the launching stream, so every bracket times its own launch only.
     saved_qs = eng.__dict__.get("_qstream")
     eng._qstream = torch.cuda.current_stream(dev)
@@ -360,22 +364,21 @@ def _roofline_dicts(rec, prof_ms, peaks, peak_src, fp16, what):
     conv_peak = peaks["bf16_tflops_sustained"] if fp16 else tf32_peak
     ach = conv_fl / (conv_ms / 1e3) / 1e12
     traffic, traffic_launch = _measured_traffic(fp16)
-    roof = {"kernel": f"conv_gemm_persistent_kernel (tcgen05 kind::{'f16' if fp16 else 'tf32'} implicit GEMM, all conv layers of the step)",
+    roof = {"kernel": f"conv_gemm_kernel (wgmma {'f16' if fp16 else 'tf32'} implicit GEMM, all conv layers of the step)",
             "bound": "tensor", "achieved": ach, "peak": conv_peak, "unit": "TFLOP/s", "frac": ach / conv_peak,
-            # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel from this round's
-            # `ncu --set full` capture (profiles/r02_traffic.json); null when no capture of the current kernels exists
+            # DRAM bytes of ONE launch of the dominant kernel from a committed capture; null when none exists
             "traffic": traffic, "traffic_launch": traffic_launch,
             "launches": len(rec["conv"]), "avg_launch_us": 1e3 * conv_ms / max(1, len(rec["conv"])),
             "share_of_step": conv_ms / prof_ms, "measured_on": what,
-            "peak_source": (f"{peak_src}: sustained dense bf16 {peaks['bf16_tflops_sustained']:.0f} (kind::f16 issues at the bf16 rate)" if fp16 else
-                            f"{peak_src}: TF32 dense = sustained bf16 {peaks['bf16_tflops_sustained']:.0f} / 2 (kind::tf32 issues at half the bf16 rate)"),
+            "peak_source": (f"{peak_src}: dense bf16 {peaks['bf16_tflops_sustained']:.0f} (fp16 wgmma issues at the bf16 rate)" if fp16 else
+                            f"{peak_src}: TF32 dense = bf16 {peaks['bf16_tflops_sustained']:.0f} / 2 (tf32 wgmma issues at half the bf16 rate)"),
             "note": "event-bracketed eager launches, the batched query pass issued on the launching stream for this pass "
                     "(no cross-stream contention inside a bracket): durations include launch gaps, so this is a lower bound; "
                     "share_of_step = bracketed time / GPU time of the same pass"}
     mr_ms = sum(a.elapsed_time(b) for a, b, _, _ in rec["memread"])
     mr_fl = sum(f for _, _, f, _ in rec["memread"])
     mr_by = sum(by for _, _, _, by in rec["memread"])
-    roof_mr = {"kernel": "memory_read (candidate pass on tcgen05 + exact selection / read-out)", "bound": "tensor",
+    roof_mr = {"kernel": "memory_read (candidate pass on wgmma tf32 + exact selection / read-out)", "bound": "tensor",
                "achieved": mr_fl / (mr_ms / 1e3) / 1e12, "peak": tf32_peak, "unit": "TFLOP/s",
                "frac": mr_fl / (mr_ms / 1e3) / 1e12 / tf32_peak, "hbm_gbs": mr_by / (mr_ms / 1e3) / 1e9,
                "hbm_frac": mr_by / (mr_ms / 1e3) / 1e9 / peaks["hbm_gbs"], "launches": len(rec["memread"]),
@@ -509,7 +512,19 @@ def run_ours(args, cfgd, cfg_name):
                     self.checksums[j] += int(m.sum(dtype="int64"))
             self.results = []
 
-    def timed_region(lanes, C, L, mem_profile, nsteps, warm):
+    def dump_outputs(lanes, cores, out_dir):
+        """The last timed step's results, per clip: a fixed seeded sample of the masks interact() returned and
+        of the session's probabilities, as float32 (at most 2 x 1 MB per clip, 64 MB in all)."""
+        os.makedirs(out_dir, exist_ok=True)
+        n_sample = min(1 << 18, (64 << 20) // (4 * 2 * sum(len(ln.clips) for ln in lanes)))
+        for ln, cs in zip(lanes, cores):
+            for j, (c, core) in enumerate(zip(ln.clips, cs)):
+                for name, arr in (("masks", np.asarray(ln.results[-1][j])), ("prob", core.prob.float().cpu().numpy())):
+                    flat = arr.reshape(-1)
+                    idx = np.random.default_rng(c).integers(0, flat.size, n_sample) if flat.size > n_sample else np.arange(flat.size)
+                    np.save(os.path.join(out_dir, f"{name}_c{c}.npy"), flat[idx].astype(np.float32))
+
+    def timed_region(lanes, C, L, mem_profile, nsteps, warm, dump_dir=None):
         cores = [[mivos_b200.InferenceCore(ln.net, ln.fuse, ln.images_l[j], K, mem_profile=mem_profile, mem_freq=MEM_FREQ,
                                            device=dev) for j in range(L)] for ln in lanes]
         for ln, cs in zip(lanes, cores):  # warm-up lane by lane (graph capture is single-threaded)
@@ -536,6 +551,8 @@ def run_ours(args, cfgd, cfg_name):
         wall = time.perf_counter() - t0
         ms = e0.elapsed_time(e1)
         launches = _lib.load().mivos_launch_count() - l0
+        if dump_dir:
+            dump_outputs(lanes, cores, dump_dir)
         for ln in lanes:
             ln.take_checksum()
         step_ms = [[round(1e3 * x, 2) for x in ln.step_wall] for ln in lanes]
@@ -544,13 +561,13 @@ def run_ours(args, cfgd, cfg_name):
         del cores
         return {"ms": sharding.max_over_ranks(ms, dev), "launches": launches, "checksum": sum(per_clip), "wall": wall, "step_ms": step_ms}
 
-    def measure(act, C, L, nsteps, warm, sample_clocks=False):
+    def measure(act, C, L, nsteps, warm, sample_clocks=False, dump_dir=None):
         """value (mem_profile 0) and e2e (mem_profile 1) of one (element type, lanes, lock-step) setting."""
         lanes = [Lane(i, C, L, act) for i in range(C)]
         sampler = ClockSampler(local) if sample_clocks else None
         if sampler:
             sampler.start()
-        r0 = timed_region(lanes, C, L, 0, nsteps, warm)
+        r0 = timed_region(lanes, C, L, 0, nsteps, warm, dump_dir)
         clocks = sampler.stop() if sampler else None
         r1 = timed_region(lanes, C, L, 1, nsteps, max(1, warm // 3))
         n = world * C * L * frames * nsteps
@@ -560,7 +577,7 @@ def run_ours(args, cfgd, cfg_name):
 
     C = max(1, args.clips_per_gpu if args.clips_per_gpu is not None else cfgd["lanes"])
     L = max(1, args.lockstep if args.lockstep is not None else cfgd["lockstep"])
-    head, lanes = measure(ACT_DTYPE, C, L, args.steps, args.warmup, sample_clocks=True)
+    head, lanes = measure(ACT_DTYPE, C, L, args.steps, args.warmup, sample_clocks=True, dump_dir=args.dump_outputs)
     h2d = world * C * L * (T * 3 * nh * nw * 4 + len(inter) * (K + 1) * Hh * Ww * 4)  # whole job, like `value`
     d2h = world * C * L * len(inter) * T * Hh * Ww
 
@@ -674,6 +691,8 @@ def main():
     ap.add_argument("--skip-extras", action="store_true", help="no single-session / other-dtype measurements")
     ap.add_argument("--skip-cuda-eager", action="store_true", help="no PyTorch-eager CUDA comparator")
     ap.add_argument("--skip-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a fixed sample of what the last timed step returned (per clip: masks, probabilities) as DIR/<name>.npy")
     ap.add_argument("--act", default=os.environ.get("MIVOS_ACT_DTYPE", DEFAULT_ACT), choices=["tf32", "fp16"],
                     help="convolution operand / activation type of the headline measurement (fp16 = the reference GUI's autocast "
                          "precision; the other type is measured beside it)")
@@ -681,7 +700,7 @@ def main():
                     help="concurrent lanes per GPU (own network object, CUDA stream and Python thread each); default per configuration")
     ap.add_argument("--lockstep", type=int, default=(int(os.environ["MIVOS_LOCKSTEP"]) if "MIVOS_LOCKSTEP" in os.environ else None),
                     help="clips each lane advances in lock-step as ONE batch through the conv layers (mivos_b200.LockstepSession); "
-                         "1 = off; default per configuration (cfg2: 3 lanes x 4 clips)")
+                         "1 = off; default per configuration (cfg2: 2 lanes x 4 clips)")
     args = ap.parse_args()
     global ACT_DTYPE
     ACT_DTYPE = torch.float16 if args.act == "fp16" else torch.float32

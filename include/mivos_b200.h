@@ -1,4 +1,4 @@
-/* mivos_b200 — C ABI of the B200-native mask-propagation hot path.
+/* mivos_b200 — C ABI of the H100-native mask-propagation hot path.
  *
  * The reference (hkchengrex/MiVOS) has no FFI: its hot path is PyTorch library calls made from
  * `PropagationNetwork` / `InferenceCore` (SURVEY.md §8b).  This header is the boundary a
@@ -39,7 +39,7 @@ enum {
   MIVOS_OK = 0,
   MIVOS_ERR_INVALID = -1,  /* bad argument (shape, alignment, null pointer) */
   MIVOS_ERR_CUDA = -2,     /* a CUDA runtime/driver call failed */
-  MIVOS_ERR_DEVICE = -3,   /* not an sm_100 device */
+  MIVOS_ERR_DEVICE = -3,   /* not an sm_90 device */
   MIVOS_ERR_KERNEL = -4    /* a kernel raised its error flag (bounded wait expired, overflow) */
 };
 
@@ -51,7 +51,7 @@ enum {
                                   skip_n (upsample2x_add) */
 MIVOS_API int mivos_abi_version(void);
 MIVOS_API const char* mivos_last_error(void);
-/* MIVOS_OK iff the current device is compute capability 10.x (there is no other code path). */
+/* MIVOS_OK iff the current device is compute capability 9.0 (there is no other code path). */
 MIVOS_API int mivos_check_device(void);
 /* Reads (and clears) the device-side error flag set by kernels; synchronises `stream`. */
 MIVOS_API int mivos_poll_kernel_error(mivos_stream_t stream, int* code_out);
@@ -74,7 +74,7 @@ MIVOS_API int mivos_store_words(int64_t* dst64, int n64, const int64_t* vals64, 
 MIVOS_API int mivos_copy_segments(const int64_t* fixed, const int64_t* dyn, const int64_t* bytes, int n,
                         int dyn_is_src, int64_t max_bytes, mivos_stream_t stream);
 
-/* Convolution as implicit GEMM on tcgen05 (TF32 in, FP32 accumulate) -------------------------
+/* Convolution as implicit GEMM on wgmma (TF32 in, FP32 accumulate) ----------------------------
  * Replaces nn.Conv2d (+ eval BatchNorm2d folded into weight/bias, + ReLU, + residual add) as
  * used by model/propagation/modules.py:15-35,38-89,92-114, mod_resnet.py:76-112,
  * prop_net.py:14-31 and model/fusion_net.py:8-50.
@@ -87,7 +87,7 @@ MIVOS_API int mivos_copy_segments(const int64_t* fixed, const int64_t* dyn, cons
  * (64 for fp16 operands), cout_pad a multiple of 32.  Weight is packed [taps][cout_pad][cin_pad]
  * in the operand type, bias [cout_pad] is always fp32.  Activations may be fp32 (TF32 MMAs) or
  * fp16 (the precision the reference GUI itself runs in: torch.cuda.amp.autocast,
- * interactive_gui.py:990); accumulation is always fp32 in TMEM.                                  */
+ * interactive_gui.py:990); accumulation is always fp32.                                          */
 typedef struct {
   const void* in;  /* fp32 or fp16 (in_f16) */
   int64_t in_rows; /* rows of the input matrix that exist (TMA zero-fills beyond) */
@@ -212,12 +212,12 @@ MIVOS_API int mivos_memory_read(const float* bank_k, const float* bank_v, int64_
                       void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
                       int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
                       int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
-/* Diagnostic, synchronising: candidate statistics of the last tcgen05-path read in `workspace`:
+/* Diagnostic, synchronising: candidate statistics of the last tensor-core-path read in `workspace`:
  * out[0] total candidates, out[1] max per (object, query), out[2] queries served by the exact
  * fallback, out[3] splits of the memory axis.                                                    */
 MIVOS_API int mivos_memory_read_stats(const void* workspace, int k_objects, int64_t slots, int hw, int top_k,
                             int64_t* out);
-enum { MIVOS_MEMREAD_AUTO = 0, MIVOS_MEMREAD_EXACT_SIMT = 1, MIVOS_MEMREAD_TCGEN05 = 2 };
+enum { MIVOS_MEMREAD_AUTO = 0, MIVOS_MEMREAD_EXACT_SIMT = 1, MIVOS_MEMREAD_TCGEN05 = 2 };  /* (name kept for ABI stability: the tensor-core candidate path, wgmma on sm_90) */
 
 /* Decoder tail + soft aggregation — prop_net.py:30 (bilinear x4, align_corners=False),
  * prop_net.py:181 (sigmoid) and aggregate_wbg (aggregate.py:22-37, keep_bg=True).

@@ -5,9 +5,9 @@ Public surface (mirrors the reference's import paths through the top-level shim 
 ``util.tensor_util``):
     InferenceCore, PropagationNetwork, FusionNet, aggregate_wbg, aggregate_sbg,
     pad_divide_by, unpad, unpad_3dim
-Everything computes through ``libmivos_b200.so`` (hand-written sm_100a CUDA behind the C ABI in
+Everything computes through ``libmivos_b200.so`` (hand-written sm_90a CUDA behind the C ABI in
 include/mivos_b200.h).  There is no CPU or PyTorch fallback: ops raise if the library is missing
-or the device is not a B200.
+or the device is not an H100.
 """
 from .aggregate import aggregate_sbg, aggregate_wbg  # noqa: F401
 from .attn_network import AttentionReadNetwork  # noqa: F401

@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI declared in include/mivos_b200.h.
 
 The shared library is built in-tree by ``__graft_entry__.build()`` / ``make -C mivos_b200/csrc``.
-There is no fallback: if the library is missing, or the device is not sm_100, every op raises.
+There is no fallback: if the library is missing, or the device is not sm_90, every op raises.
 """
 from __future__ import annotations
 
@@ -134,7 +134,7 @@ _device_ok = False
 
 
 def lib() -> C.CDLL:
-    """Library handle for launching work: also verifies the current device is sm_100."""
+    """Library handle for launching work: also verifies the current device is sm_90."""
     global _device_ok
     l = load()
     if not _device_ok:

@@ -174,7 +174,7 @@ extern "C" MIVOS_API int mivos_attention_map(const float* mk, const float* qk, i
   MIVOS_CUDA_OK(cudaGetLastError());
   const int64_t total = 2ll * hw * 256;
   int64_t g = (total + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > num_sms() * 16) g = num_sms() * 16;
   launch_pdl(upsample16_kernel, static_cast<unsigned>(g), 256, 0, stream, maps, h16, w16, out);
   g_launches.fetch_add(1);
   MIVOS_CUDA_OK(cudaGetLastError());

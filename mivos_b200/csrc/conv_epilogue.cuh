@@ -1,211 +1,113 @@
-// Epilogue of the implicit-GEMM convolution kernels: one 32-row x 32-column block of the fp32
-// accumulator per warp per call.
+// Epilogue of the implicit-GEMM convolution kernel: one 32-row x 32-column block of the fp32
+// accumulator tile per warp per call.
 //
-// tcgen05.ld hands every thread ONE output row (TMEM lane) and 32 consecutive columns.  Storing
-// from that layout makes each warp-wide 16-byte store touch 32 different cache lines (a 16-byte
-// piece of each) and the residual loads likewise.  So the block is transposed through a padded
-// shared-memory tile (row stride 36 floats: conflict-free for both the row-wise 16-byte writes
-// and the segment-wise reads) and all global traffic — residual read, primary store, optional
-// ReLU copy — is issued as full 128-byte row segments: a warp instruction covers 4 rows x 128
-// contiguous bytes.  The residual segments of the whole block (8 independent 16-byte loads per
-// lane) are requested BEFORE the transpose, so their L2/HBM latency overlaps the shared-memory
-// round trip instead of being paid once per row group (measured: the 1x1 expansion convs
-// 64->256 @1/4, 128->512 @1/8, 256->1024 @1/16, whose cost is all output + residual traffic,
-// spent ~7k cycles per block waiting on eight serialised residual round trips).
+// The MMA warpgroups park their accumulator fragments in a row-major shared-memory tile; the
+// epilogue reads it back segment-wise, so all global traffic — residual read, primary store,
+// optional ReLU copy — is issued as full row segments: a warp instruction covers 4 rows x 32
+// contiguous channels.  The residual segments of the whole block (8 independent loads per lane)
+// are requested BEFORE the accumulator reads, so their L2/HBM latency overlaps them instead of
+// being paid once per row group.
 #pragma once
 #include <cuda_fp16.h>
 
-constexpr int kStgStride = 36;                         // floats per staged row (32 + 4 pad)
-constexpr int kStgBytesPerWarp = 32 * kStgStride * 4;  // 4608 B
-
-// v        : the thread's 32 accumulator columns (raw bits) for row (row0 + lane)
-// stg      : this warp's staging tile
+// acc      : the accumulator tile in shared memory, row r of this block at acc[r * stride]
 // interior : ballot mask over the warp's 32 rows (bit r set = row row0+r is an interior pixel)
 // ncol0    : absolute output channel of column 0 of this block
-__device__ __forceinline__ void conv_epilogue_block(const uint32_t (&v)[32], float* stg, const int lane,
+__device__ __forceinline__ void conv_epilogue_block(const float* acc, const int stride, const int lane,
                                                     const int64_t row0, const uint32_t interior,
                                                     const int ncol0, const ConvParams& p) {
   const int nvalid = p.cout - ncol0;  // real output channels in this block (warp-uniform)
-  const int c4 = lane & 7;            // which 16-byte piece of the 128-byte row segment
+  if (nvalid <= 0 || interior == 0u) return;
+  const int c4 = lane & 7;            // which 4-channel piece of the 32-channel row segment
   const int rsub = lane >> 3;         // 0..3: row within the group of 4 rows one instruction covers
   const bool full = nvalid >= 32;
 
-  // 0. residual prefetch: 8 independent loads per lane (16 bytes fp32 / 8 bytes fp16), in flight
-  //    during steps 1-2
-  float4 res[8];
-  if (full && p.residual && interior != 0u) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int rr = i * 4 + rsub;
-      res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if ((interior >> rr) & 1u) {
-        const int64_t off = (row0 + rr) * p.res_cstride + p.res_coff + ncol0 + c4 * 4;
-        if (p.f16_out) {
-          const uint2 u = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const __half*>(p.residual) + off));
-          const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
-          const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
-          res[i] = make_float4(lo.x, lo.y, hi.x, hi.y);
-        } else {
-          res[i] = __ldg(reinterpret_cast<const float4*>(p.residual + off));
-        }
-      }
-    }
-  }
-  // 1. row-per-thread -> shared (8 x STS.128)
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    *reinterpret_cast<uint4*>(stg + lane * kStgStride + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-  }
-  __syncwarp();
-  if (nvalid > 0 && interior != 0u) {
-    if (full) {
-      const float4 b = *reinterpret_cast<const float4*>(p.bias + ncol0 + c4 * 4);
+  if (full) {
+    float4 res[8];
+    if (p.residual) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int rr = i * 4 + rsub;
-        if (!((interior >> rr) & 1u)) continue;
-        const float4 a = *reinterpret_cast<const float4*>(stg + rr * kStgStride + c4 * 4);
-        const int64_t row = row0 + rr;
-        float4 o = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-        if (p.residual) {
-          o.x += res[i].x; o.y += res[i].y; o.z += res[i].z; o.w += res[i].w;
-        }
-        if (p.relu) {
-          o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-        }
-        if (p.f16_out) {
-          // fp16 HALO output: round-to-nearest-even conversion, 8-byte stores (64 B per row segment)
-          __half2 h01 = __floats2half2_rn(o.x, o.y), h23 = __floats2half2_rn(o.z, o.w);
-          uint2 u;
-          u.x = *reinterpret_cast<uint32_t*>(&h01);
-          u.y = *reinterpret_cast<uint32_t*>(&h23);
-          *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + row * p.out_cstride + p.out_coff + ncol0 + c4 * 4) = u;
-          if (p.out_relu) {
-            h01 = __floats2half2_rn(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
-            h23 = __floats2half2_rn(fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
-            u.x = *reinterpret_cast<uint32_t*>(&h01);
-            u.y = *reinterpret_cast<uint32_t*>(&h23);
-            *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out_relu) + row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c4 * 4) = u;
-          }
-          continue;
-        }
-        if (p.round_tf32) {
-          o.x = rna_tf32(o.x); o.y = rna_tf32(o.y); o.z = rna_tf32(o.z); o.w = rna_tf32(o.w);
-        }
-        *reinterpret_cast<float4*>(p.out + row * p.out_cstride + p.out_coff + ncol0 + c4 * 4) = o;
-        if (p.out_relu) {
-          const float4 o2 = make_float4(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f), fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
-          *reinterpret_cast<float4*>(p.out_relu + row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c4 * 4) = o2;
-        }
-      }
-    } else {
-      // ragged channel tail (e.g. decoder.pred: one real output channel): element-wise
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int rr = i * 4 + rsub;
-        if (!((interior >> rr) & 1u)) continue;
-        const int64_t row = row0 + rr;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int c = c4 * 4 + e;
-          if (c < nvalid) {
-            float o = stg[rr * kStgStride + c] + p.bias[ncol0 + c];
-            if (p.f16_out) {
-              if (p.residual) o += __half2float(reinterpret_cast<const __half*>(p.residual)[row * p.res_cstride + p.res_coff + ncol0 + c]);
-              if (p.relu) o = fmaxf(o, 0.f);
-              reinterpret_cast<__half*>(p.out)[row * p.out_cstride + p.out_coff + ncol0 + c] = __float2half_rn(o);
-              if (p.out_relu)
-                reinterpret_cast<__half*>(p.out_relu)[row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c] = __float2half_rn(fmaxf(o, 0.f));
-              continue;
-            }
-            if (p.residual) o += p.residual[row * p.res_cstride + p.res_coff + ncol0 + c];
-            if (p.relu) o = fmaxf(o, 0.f);
-            if (p.round_tf32) o = rna_tf32(o);
-            p.out[row * p.out_cstride + p.out_coff + ncol0 + c] = o;
-            if (p.out_relu) p.out_relu[row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c] = fmaxf(o, 0.f);
+        res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if ((interior >> rr) & 1u) {
+          const int64_t off = (row0 + rr) * p.res_cstride + p.res_coff + ncol0 + c4 * 4;
+          if (p.f16_out) {
+            const uint2 u = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const __half*>(p.residual) + off));
+            const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+            const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+            res[i] = make_float4(lo.x, lo.y, hi.x, hi.y);
+          } else {
+            res[i] = __ldg(reinterpret_cast<const float4*>(p.residual + off));
           }
         }
       }
     }
-  }
-  __syncwarp();  // the tile is reused by the next block
-}
-
-// ------------------------------------------------------------------------------------------
-// fp16 output maps: 32 rows x 64 columns per step.  A row segment is then 64 x 2 B = 128 bytes —
-// one full line per (row, step) for the residual read, the store and the optional ReLU copy; lane
-// l handles the 16-byte piece (l & 7) of rows (l >> 3) + 4 i.  Staging tile: fp32 [32][68]
-// (the sum bias + accumulator + residual is formed in fp32 and rounded to fp16 once).
-constexpr int kStg64Stride = 68;
-constexpr int kStg64BytesPerWarp = 32 * kStg64Stride * 4;  // 8704 B
-
-__device__ __forceinline__ void conv_epilogue_prefetch64(uint4 (&res)[8], const int lane, const int64_t row0,
-                                                         const uint32_t interior, const int ncol0,
-                                                         const ConvParams& p) {
-  if (!p.residual || interior == 0u) return;
-  const int c8 = lane & 7, rsub = lane >> 3;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int rr = i * 4 + rsub;
-    res[i] = make_uint4(0u, 0u, 0u, 0u);
-    if ((interior >> rr) & 1u)
-      res[i] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(p.residual) +
-                                                    (row0 + rr) * p.res_cstride + p.res_coff + ncol0 + c8 * 8));
-  }
-}
-
-// thread `lane` holds accumulator row (row0 + lane), 32 columns -> staging columns col_off..+31
-__device__ __forceinline__ void conv_epilogue_stage64(const uint32_t (&v)[32], float* stg, const int lane,
-                                                      const int col_off) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4)
-    *reinterpret_cast<uint4*>(stg + lane * kStg64Stride + col_off + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-}
-
-__device__ __forceinline__ uint4 pack8_half(const float (&o)[8]) {
-  const __half2 a = __floats2half2_rn(o[0], o[1]), b = __floats2half2_rn(o[2], o[3]);
-  const __half2 c = __floats2half2_rn(o[4], o[5]), d = __floats2half2_rn(o[6], o[7]);
-  return make_uint4(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b),
-                    *reinterpret_cast<const uint32_t*>(&c), *reinterpret_cast<const uint32_t*>(&d));
-}
-
-__device__ __forceinline__ void conv_epilogue_store64(float* stg, const int lane, const int64_t row0,
-                                                      const uint32_t interior, const int ncol0, const ConvParams& p,
-                                                      const uint4 (&res)[8]) {
-  __syncwarp();
-  if (interior != 0u) {
-    const int c8 = lane & 7, rsub = lane >> 3;
-    const float4 b0 = *reinterpret_cast<const float4*>(p.bias + ncol0 + c8 * 8);
-    const float4 b1 = *reinterpret_cast<const float4*>(p.bias + ncol0 + c8 * 8 + 4);
+    const float4 b = *reinterpret_cast<const float4*>(p.bias + ncol0 + c4 * 4);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int rr = i * 4 + rsub;
       if (!((interior >> rr) & 1u)) continue;
-      const float4 a0 = *reinterpret_cast<const float4*>(stg + rr * kStg64Stride + c8 * 8);
-      const float4 a1 = *reinterpret_cast<const float4*>(stg + rr * kStg64Stride + c8 * 8 + 4);
-      float o[8] = {a0.x + b0.x, a0.y + b0.y, a0.z + b0.z, a0.w + b0.w, a1.x + b1.x, a1.y + b1.y, a1.z + b1.z, a1.w + b1.w};
+      const float4 a = *reinterpret_cast<const float4*>(acc + rr * stride + c4 * 4);
+      const int64_t row = row0 + rr;
+      float4 o = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
       if (p.residual) {
-        const uint32_t w[4] = {res[i].x, res[i].y, res[i].z, res[i].w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&w[e]));
-          o[2 * e] += t.x;
-          o[2 * e + 1] += t.y;
-        }
+        o.x += res[i].x; o.y += res[i].y; o.z += res[i].z; o.w += res[i].w;
       }
       if (p.relu) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
+        o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
       }
-      const int64_t row = row0 + rr;
-      *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.out) + row * p.out_cstride + p.out_coff + ncol0 + c8 * 8) = pack8_half(o);
+      if (p.f16_out) {
+        // fp16 HALO output: round-to-nearest-even conversion, 8-byte stores (64 B per row segment)
+        __half2 h01 = __floats2half2_rn(o.x, o.y), h23 = __floats2half2_rn(o.z, o.w);
+        uint2 u;
+        u.x = *reinterpret_cast<uint32_t*>(&h01);
+        u.y = *reinterpret_cast<uint32_t*>(&h23);
+        *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + row * p.out_cstride + p.out_coff + ncol0 + c4 * 4) = u;
+        if (p.out_relu) {
+          h01 = __floats2half2_rn(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
+          h23 = __floats2half2_rn(fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
+          u.x = *reinterpret_cast<uint32_t*>(&h01);
+          u.y = *reinterpret_cast<uint32_t*>(&h23);
+          *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out_relu) + row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c4 * 4) = u;
+        }
+        continue;
+      }
+      if (p.round_tf32) {
+        o.x = rna_tf32(o.x); o.y = rna_tf32(o.y); o.z = rna_tf32(o.z); o.w = rna_tf32(o.w);
+      }
+      *reinterpret_cast<float4*>(p.out + row * p.out_cstride + p.out_coff + ncol0 + c4 * 4) = o;
       if (p.out_relu) {
+        const float4 o2 = make_float4(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f), fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
+        *reinterpret_cast<float4*>(p.out_relu + row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c4 * 4) = o2;
+      }
+    }
+    return;
+  }
+  // ragged channel tail (e.g. decoder.pred: one real output channel): element-wise
 #pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
-        *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.out_relu) + row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c8 * 8) = pack8_half(o);
+  for (int i = 0; i < 8; ++i) {
+    const int rr = i * 4 + rsub;
+    if (!((interior >> rr) & 1u)) continue;
+    const int64_t row = row0 + rr;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int c = c4 * 4 + e;
+      if (c < nvalid) {
+        float o = acc[rr * stride + c] + p.bias[ncol0 + c];
+        if (p.f16_out) {
+          if (p.residual) o += __half2float(reinterpret_cast<const __half*>(p.residual)[row * p.res_cstride + p.res_coff + ncol0 + c]);
+          if (p.relu) o = fmaxf(o, 0.f);
+          reinterpret_cast<__half*>(p.out)[row * p.out_cstride + p.out_coff + ncol0 + c] = __float2half_rn(o);
+          if (p.out_relu)
+            reinterpret_cast<__half*>(p.out_relu)[row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c] = __float2half_rn(fmaxf(o, 0.f));
+          continue;
+        }
+        if (p.residual) o += p.residual[row * p.res_cstride + p.res_coff + ncol0 + c];
+        if (p.relu) o = fmaxf(o, 0.f);
+        if (p.round_tf32) o = rna_tf32(o);
+        p.out[row * p.out_cstride + p.out_coff + ncol0 + c] = o;
+        if (p.out_relu) p.out_relu[row * p.out_relu_cstride + p.out_relu_coff + ncol0 + c] = fmaxf(o, 0.f);
       }
     }
   }
-  __syncwarp();  // the tile is reused by the next step
 }
-

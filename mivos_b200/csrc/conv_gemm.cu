@@ -1,23 +1,28 @@
-// Implicit-GEMM convolution on tcgen05 (kind::tf32, FP32 accumulate in TMEM), sm_100a only.
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma, TF32 or FP16 operands, FP32
+// accumulate), sm_90a only.
 //
 // Replaces every nn.Conv2d(+BatchNorm eval)(+ReLU)(+residual) of the reference's propagation
 // path: model/propagation/modules.py:15-35 (ResBlock), :38-89 (encoders), :92-114 (Upsample,
 // KeyValue), mod_resnet.py:76-112 (Bottleneck), prop_net.py:14-31 (Decoder),
 // model/fusion_net.py:8-50 (FusionNet).
 //
-// Activations live in HALO layout (include/mivos_b200.h): a flattened [rows, C] fp32 matrix with
-// a zero one-pixel border per image, so tap (dy,dx) of a 3x3/pad-1 conv is the same matrix
-// shifted by dy*(W+2)+dx rows.  One CTA computes a 128-row x BN-column output tile:
-//   warp 0   : TMA producer  - per (tap, 32-channel k-block) loads A box {32ch x 128 rows} at the
-//              shifted row and B box {32ch x BN rows} of the packed weights, 128B-swizzled
-//   warp 1   : allocates TMEM, single elected thread issues 4 x tcgen05.mma (K=8) per k-block,
-//              tcgen05.commit releases the smem stage / signals the accumulator
-//   warps 2-5: epilogue - tcgen05.ld 32 columns at a time, + bias (+ residual) (ReLU), vector
-//              stores to interior rows only (the halo stays zero)
-// Roofline: tensor pipe (TF32); algorithmic flops = 2 * rows_interior * taps*cin * cout.
+// Activations live in HALO layout (include/mivos_b200.h): a flattened [rows, C] matrix with a
+// zero one-pixel border per image, so tap (dy,dx) of a 3x3/pad-1 conv is the same matrix shifted
+// by dy*(W+2)+dx rows.  One CTA computes a 128-row x BN-column output tile (or one K range of it
+// under split-K):
+//   warpgroup 0 : one thread is the TMA producer - per (tap, 128-byte k-block) it loads the A box
+//                 {k-block x 128 rows} at the shifted row and the B box {k-block x BN rows} of the
+//                 packed weights, 128B-swizzled, into a ring of STAGES stages
+//   warpgroups 1-2 : rows 0-63 / 64-127 of the tile: 4 x wgmma (K = 32 bytes each) per k-block
+//                 into a register accumulator; a stage is handed back once the wgmmas that read it
+//                 have completed (one arrival per warp)
+//   epilogue   : the accumulators are parked in a row-major shared-memory tile (over the drained
+//                 ring), then every warp stores 32 x 32 blocks: + bias (+ residual) (ReLU), to
+//                 interior rows only (the halo stays zero)
+// Roofline: tensor pipe (TF32 / FP16); algorithmic flops = 2 * rows_interior * taps*cin * cout.
 #include "host_util.h"
 #include "pdl.cuh"
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 #include <atomic>
 #include <stdlib.h>
@@ -56,9 +61,9 @@ struct ConvParams {
   int* err;
 };
 
-// round-to-nearest (ties away) to TF32 precision: the tensor core TRUNCATES fp32 operands to
-// TF32 (measured on B200, profiles/r01_probe1_first_contact.log), which would bias every layer
-// by about -1e-3; storing activations pre-rounded makes that truncation a no-op.
+// round-to-nearest (ties away) to TF32 precision: the tensor core reads only the TF32 bits of fp32
+// operands (truncation), which would bias every layer by about -1e-3; storing activations
+// pre-rounded makes that truncation a no-op.
 __device__ __forceinline__ float rna_tf32(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
@@ -67,131 +72,153 @@ __device__ __forceinline__ float rna_tf32(float x) {
 
 #include "conv_epilogue.cuh"
 
-template <int BN, int STAGES>
-struct SmemLayout {
-  static constexpr int B_BYTES = BN * BK * 4;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
-  static constexpr int STG_OFF = (BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 127) & ~127;  // 16B-aligned staging
-  static constexpr int TOTAL = STG_OFF + 4 * kStgBytesPerWarp;
-};
+constexpr int kConvThreads = 384;  // producer warpgroup + two MMA / epilogue warpgroups
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(192, 1)
+struct SmemLayout {
+  static constexpr int B_BYTES = BN * 128;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  // accumulator tile [128][BN + 8] fp32: the pad makes the fragment stores (8-byte pieces of 4 rows per
+  // half-warp) conflict-free; it reuses the ring, which is drained when the tile is written
+  static constexpr int ACC_STRIDE = BN + 8;
+  static constexpr int ACC_BYTES = BM * ACC_STRIDE * 4;
+  static constexpr int BAR_OFF = ((RING_BYTES > ACC_BYTES ? RING_BYTES : ACC_BYTES) + 7) & ~7;
+  static constexpr int TOTAL = BAR_OFF + 2 * STAGES * 8;
+};
+
+template <int BN, int STAGES, bool F16>
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const ConvParams p) {
+                 const ConvParams p, const int m_tiles) {
   using L = SmemLayout<BN, STAGES>;
-  constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem base is only guaranteed 16B aligned; round up to the 1024B the swizzle needs
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int64_t m0 = static_cast<int64_t>(blockIdx.x) * BM;
-  const int n0 = blockIdx.y * BN;
+  const int mt = blockIdx.x, nt = blockIdx.y, split = blockIdx.z;
+  const int64_t m0 = static_cast<int64_t>(mt) * BM;
+  const int n0 = nt * BN;
   const int iters = p.taps * p.kblocks;
+  const int S = p.splits;
+  const int j0 = static_cast<int>(static_cast<int64_t>(split) * iters / S);
+  const int j1 = static_cast<int>(static_cast<int64_t>(split + 1) * iters / S);
 
-  if (warp == 0 && lane == 0) {
-    tc05::prefetch_tmap(&tmA);
-    tc05::prefetch_tmap(&tmB);
+  if (threadIdx.x == 0) {
+    sm90::prefetch_tmap(&tmA);
+    sm90::prefetch_tmap(&tmB);
     for (int s = 0; s < STAGES; ++s) {
-      tc05::mbar_init(&full_bar[s], 1);
-      tc05::mbar_init(&empty_bar[s], 1);
+      sm90::mbar_init(&full_bar[s], 1);
+      sm90::mbar_init(&empty_bar[s], 8);  // one arrival per MMA warp
     }
-    tc05::mbar_init(tmem_full_bar, 1);
-    tc05::fence_barrier_init();
+    sm90::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc05::tmem_alloc<TMEM_COLS>(tmem_slot);
-  }
-  tc05::fence_before_sync();
   __syncthreads();
-  tc05::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();  // prologue above ran under the previous kernel's tail (pdl.cuh)
+  // everything above touched only shared memory and the kernel parameters: it ran under the previous
+  // kernel's tail (pdl.cuh); from here on global memory is read and written
+  pdl_wait();
 
-  if (warp == 0) {
-    if (tc05::elect_one()) {
+  if (warp < 4) {
+    sm90::setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       const int wp = p.w + 2;
-      for (int it = 0; it < iters; ++it) {
+      for (int j = j0, it = 0; j < j1; ++j, ++it) {
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
-        const int t = it / p.kblocks;
-        const int kb = it - t * p.kblocks;
+        const int t = j / p.kblocks;
+        const int kb = j - t * p.kblocks;
         int64_t row = m0;
         if (p.taps == 9) row += static_cast<int64_t>(t / 3 - 1) * wp + (t % 3 - 1);
-          else if (p.taps == 4) row += static_cast<int64_t>(t - 2) * wp;  // vertical taps dy = -2..1 (space-to-depth stem)
-        tc05::mbar_wait(&empty_bar[s], ph ^ 1, p.err, 101);
-        tc05::mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
+        else if (p.taps == 4) row += static_cast<int64_t>(t - 2) * wp;  // vertical taps dy = -2..1 (space-to-depth stem)
+        sm90::mbar_wait(&empty_bar[s], ph ^ 1, p.err, 101);
+        sm90::mbar_arrive_expect_tx(&full_bar[s], L::STAGE_BYTES);
         uint8_t* sa = smem + s * L::STAGE_BYTES;
-        tc05::tma_load_2d(sa, &tmA, &full_bar[s], p.in_coff + kb * BK, static_cast<int32_t>(row));
-        tc05::tma_load_2d(sa + A_BYTES, &tmB, &full_bar[s], kb * BK, t * p.cout_pad + n0);
+        sm90::tma_load_2d(sa, &tmA, &full_bar[s], p.in_coff + kb * p.bk, static_cast<int32_t>(row));
+        sm90::tma_load_2d(sa + A_BYTES, &tmB, &full_bar[s], kb * p.bk, t * p.cout_pad + n0);
       }
     }
-  } else if (warp == 1) {
-    if (tc05::elect_one()) {
-      constexpr uint32_t idesc = tc05::make_idesc_tf32(BM, BN);
-      for (int it = 0; it < iters; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        tc05::mbar_wait(&full_bar[s], ph, p.err, 102);
-        tc05::fence_after_sync();
-        const uint32_t sa = tc05::smem_u32(smem + s * L::STAGE_BYTES);
-        const uint64_t da = tc05::make_desc_sw128(sa);
-        const uint64_t db = tc05::make_desc_sw128(sa + A_BYTES);
+    return;
+  }
+
+  sm90::setmaxnreg_inc<232>();
+  const int wg = warp / 4 - 1;  // 0: rows 0-63, 1: rows 64-127
+  const int tw = threadIdx.x - 128 * (wg + 1);
+  float acc[BN / 2];
 #pragma unroll
-        for (int k = 0; k < BK / 8; ++k) {
-          // +32 bytes per K=8 step inside the 128B swizzle row -> +2 in 16-byte address units
-          tc05::umma_tf32_ss(tmem_base, da + 2 * k, db + 2 * k, idesc, (it | k) != 0 ? 1u : 0u);
-        }
-        tc05::umma_commit(&empty_bar[s]);
-      }
-      tc05::umma_commit(tmem_full_bar);
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int prev = -1;
+  for (int j = j0, it = 0; j < j1; ++j, ++it) {
+    const int s = it % STAGES;
+    sm90::mbar_wait(&full_bar[s], (it / STAGES) & 1, p.err, 102);
+    const uint32_t sa = sm90::smem_u32(smem + s * L::STAGE_BYTES);
+    const uint64_t da = sm90::make_desc_sw128(sa + wg * 64 * 128);
+    const uint64_t db = sm90::make_desc_sw128(sa + A_BYTES);
+    sm90::wgmma_fence();
+    // a 128-byte k-block row is 4 MMA K-steps of 32 bytes in either type (8 x fp32 / 16 x fp16): +2 in 16-byte units
+#pragma unroll
+    for (int k = 0; k < 4; ++k) sm90::wgmma<BN, F16>(acc, da + 2 * k, db + 2 * k, (j != j0 || k != 0) ? 1u : 0u);
+    sm90::wgmma_commit();
+    sm90::wgmma_wait<1>();  // the previous k-block's wgmmas are done: its stage may be refilled
+    if (prev >= 0 && lane == 0) sm90::mbar_arrive(&empty_bar[prev]);
+    prev = s;
+  }
+  sm90::wgmma_wait<0>();
+  sm90::fence_acc(acc);
+
+  // both warpgroups have finished reading the ring (and every TMA write into it was waited for): the
+  // accumulator tile may overwrite it
+  sm90::named_sync(1, 256);
+  float* tile = reinterpret_cast<float*>(smem);
+  {
+    const int r = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2);
+    const int c = 2 * (tw & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(tile + r * L::ACC_STRIDE + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(tile + (r + 8) * L::ACC_STRIDE + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-  } else {
-    // ---------------- epilogue: warps 2..5 own TMEM lane quarters (warp % 4)
-    const int q = warp & 3;
-    const int64_t r = m0 + q * 32 + lane;
+  }
+  sm90::named_sync(1, 256);
+
+  // epilogue: 32-row x 32-column blocks, consumer warp cw takes blocks cw, cw + 8, ...
+  const int cw = warp - 4;
+  const int wp = p.w + 2;
+  const int64_t per_img = static_cast<int64_t>(p.h + 2) * wp;
+#pragma unroll 1
+  for (int blk = cw; blk < 4 * (BN / 32); blk += 8) {
+    const int rb = blk & 3, cb = blk >> 2;
+    const int64_t row0 = m0 + rb * 32;
+    const float* src = tile + rb * 32 * L::ACC_STRIDE + cb * 32;
+    if (S > 1) {
+      // split-K: park the fp32 partial block in the workspace [tile][split][128 rows][BN]; splitk_epilogue_kernel
+      // (next launch) sums the S partials in split order and applies bias / residual / ReLU / conversion
+      float* dst = p.sk_ws + (((static_cast<int64_t>(nt) * m_tiles + mt) * S + split) * BM + rb * 32) * BN + cb * 32;
+      const int c4 = lane & 7, rsub = lane >> 3;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int rr = i * 4 + rsub;
+        *reinterpret_cast<float4*>(dst + rr * BN + c4 * 4) = *reinterpret_cast<const float4*>(src + rr * L::ACC_STRIDE + c4 * 4);
+      }
+      continue;
+    }
+    const int64_t r = row0 + lane;
     bool interior = false;
     if (r < p.rows) {
-      const int wp = p.w + 2;
-      const int64_t per_img = static_cast<int64_t>(p.h + 2) * wp;
       const int64_t rem = r % per_img;
       const int y = static_cast<int>(rem / wp);
       const int x = static_cast<int>(rem - static_cast<int64_t>(y) * wp);
       interior = (y >= 1) && (y <= p.h) && (x >= 1) && (x <= p.w);
     }
-    tc05::mbar_wait(tmem_full_bar, 0, p.err, 103);
-    tc05::fence_after_sync();
     const uint32_t interior_mask = __ballot_sync(0xffffffffu, interior);
-    float* stg = reinterpret_cast<float*>(smem + L::STG_OFF) + q * (kStgBytesPerWarp / 4);
-    const int64_t row0 = m0 + q * 32;
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      uint32_t v[32];
-      tc05::tmem_ld32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c0, v);
-      tc05::tmem_ld_wait();
-      conv_epilogue_block(v, stg, lane, row0, interior_mask, n0 + c0, p);
-    }
-  }
-
-  tc05::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc05::fence_after_sync();
-    tc05::tmem_dealloc<TMEM_COLS>(tmem_base);
+    conv_epilogue_block(src, L::ACC_STRIDE, lane, row0, interior_mask, n0 + cb * 32, p);
   }
 }
-
-#include "conv_gemm_persistent.cuh"
 
 // Split-K second pass: out = epilogue(sum over the S parked partial tiles, in split order).
 // Partials are [tile = nt * m_tiles + mt][split][128 rows][bn] fp32 (tile order of tile_of<1>);
@@ -245,21 +272,29 @@ __global__ void splitk_epilogue_kernel(const ConvParams p, const int bn) {
   }
 }
 
-template <int BN, int STAGES>
-int launch(const mivos_conv_args* a, const CUtensorMap& tmA, const CUtensorMap& tmB,
-           const ConvParams& p, cudaStream_t stream) {
+template <int BN, int STAGES, bool F16>
+int launch(const mivos_conv_args* a, const ConvParams& p, cudaStream_t stream) {
   using L = SmemLayout<BN, STAGES>;
   constexpr int smem_bytes = L::TOTAL + 1024;  // slack for the manual 1024B alignment
+  static_assert(smem_bytes <= 232448, "stage ring exceeds the 227 KB a CTA may use");
+  auto kernel = conv_gemm_kernel<BN, STAGES, F16>;
   static bool configured = false;
   if (!configured) {
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(conv_gemm_kernel<BN, STAGES>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     configured = true;
   }
-  dim3 grid(static_cast<unsigned>(ceil_div64(p.rows, BM)), static_cast<unsigned>(a->cout_pad / BN));
-  launch_pdl(conv_gemm_kernel<BN, STAGES>, grid, 192, smem_bytes, stream, tmA, tmB, p);
+  CUtensorMap tmA, tmB;
+  const int eb = a->in_f16 ? 2 : 4;
+  int rc = encode_tmap_2d(&tmA, a->in, static_cast<uint64_t>(a->in_rows), static_cast<uint64_t>(a->in_cstride),
+                          static_cast<uint64_t>(a->in_cstride), p.bk, BM, eb);
+  if (rc != MIVOS_OK) return rc;
+  rc = encode_tmap_2d(&tmB, a->weight, static_cast<uint64_t>(a->taps) * a->cout_pad, static_cast<uint64_t>(a->cin_pad),
+                      static_cast<uint64_t>(a->cin_pad), p.bk, BN, eb);
+  if (rc != MIVOS_OK) return rc;
+  const int m_tiles = static_cast<int>(ceil_div64(p.rows, BM));
+  dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(a->cout_pad / BN), static_cast<unsigned>(p.splits));
+  MIVOS_CUDA_OK(launch_pdl(kernel, grid, kConvThreads, smem_bytes, stream, tmA, tmB, p, m_tiles));
   g_launches.fetch_add(1, std::memory_order_relaxed);
-  MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
 }
 
@@ -275,11 +310,12 @@ std::atomic<int> g_tile_override{0};
 namespace mivos {
 namespace {
 // Tile width BN in {256,128,64,32} (must divide cout_pad) and split-K factor by a small cost model
-// fitted to an on-device sweep (tools/tile_sweep.py, profiles/r01_tile_sweep_fp16.log), in
-// KB-equivalents of shared-memory ingest, the resource that bounds the main loop:
+// (tools/tile_sweep.py measures the tile widths on the device), in KB-equivalents of shared-memory
+// ingest, the resource that bounds the main loop:
 //   main loop of a tile = k-blocks x (16 KB of A + BN/8 KB of B + 6 KB fixed barrier/issue cost)
 //   epilogue of a tile  = half its output KB (+ the same again per residual read / ReLU copy)
-//   a persistent CTA runs ceil(tiles / SMs) tiles; the epilogue overlaps the next main loop.
+//   the tiles run in ceil(tiles / SMs) waves of one CTA per SM; the cost of a wave is the larger of the two
+//   terms (the CTAs of a wave are at different phases), plus the smaller one once for the last wave.
 // Pure host arithmetic on the argument block (no pointer is dereferenced, no device is touched):
 // exported as mivos_conv_plan so the choice can be unit-tested without a GPU.
 constexpr int64_t kSkCounterBytes = 65536;  // reserved head of the split-K workspace
@@ -313,15 +349,9 @@ int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits
       }
       const double rounds = static_cast<double>((tiles * sp + sms - 1) / sms);
       const double ml = kb_total / sp * (16.0 + cand / 8.0 + 6.0);
-      // epilogue of a tile: the 128-wide fp16 tiles run EIGHT epilogue warps (two per scheduler) through the TMA
-      // epilogue — measured (profiles/r02c6): a 64-channel step is a ~4k-cycle dependent chain of one warp, so the
-      // output-bound layers go twice as fast per output byte with two warps per scheduler
-      // Calibration (profiles/r02c8_tile_sweep_fp16.log, fp16 maps through the TMA epilogue): per output KB a tile
-      // costs ~11 KB-equivalents with 4 epilogue warps and ~7 with 8 — e.g. 1x1 64->256 +res @120x216 n=4:
-      // 47.5 us at BN=256, 30.4 us at BN=128 (8 warps), 49.7 us at BN=128 with 4 warps.
-      const bool f16_maps = a->in_f16 && a->out_f16;
-      const bool epi8 = f16_maps && cand == 128 && sp == 1;
-      const double ep = cand * out_kb_per_col * (f16_maps ? (epi8 ? 7.0 : 11.0) : 1.0);
+      // epilogue of a tile: half a KB-equivalent per output KB (fitted to an H100 sweep of the fp16 cfg-2 layers,
+      // tools/tile_sweep.py: every layer within 5 % of its best tile width)
+      const double ep = cand * out_kb_per_col;
       double cost = rounds * (ml > ep ? ml : ep) + (ml > ep ? ep : ml);
       if (sp > 1) cost = (ml + cand * 0.5 + 700.0) * 1.15;  // + partial write + reduce launch; must win by a margin
       if (cost < best_cost) {  // ties keep the wider tile (fewer barrier round trips per flop)
@@ -406,44 +436,20 @@ extern "C" MIVOS_API int mivos_conv_gemm(const mivos_conv_args* a, mivos_stream_
   p.sk_cnt = nullptr;
   p.sk_ws = reinterpret_cast<float*>(static_cast<uint8_t*>(a->splitk_ws) + kSkCounterBytes);
 
-  // Persistent, clustered kernel (double-buffered TMEM accumulator, operand multicast) by default;
-  // MIVOS_CONV_PERSISTENT=0 selects the one-tile-per-CTA kernel everywhere (A/B measurements).
-  static const bool allow_persistent = [] {
-    const char* e = getenv("MIVOS_CONV_PERSISTENT");
-    return !(e && e[0] == '0');
-  }();
-  MIVOS_REQUIRE(allow_persistent || (!a->in_f16 && !a->out_f16), "conv_gemm: fp16 needs the persistent kernel");
-  if (allow_persistent) {
-    int rc = MIVOS_OK;
-    switch (bn) {
-      // stage counts: as many 128-byte k-block stages as fit next to the epilogue staging tiles
-      // (4 x 4.5 KB for fp32 maps; 4 x 8.5 KB + 4 x 8 KB of residual tiles for the 64-column fp16 epilogue)
-      case 256: rc = a->in_f16 ? launch_persistent<256, 3, true>(a, p, stream) : launch_persistent<256, 4, false>(a, p, stream); break;
-      case 128: rc = a->in_f16 ? launch_persistent<128, 4, true>(a, p, stream) : launch_persistent<128, 6, false>(a, p, stream); break;
-      case 64:  rc = a->in_f16 ? launch_persistent<64, 6, true>(a, p, stream) : launch_persistent<64, 8, false>(a, p, stream); break;
-      default:  rc = a->in_f16 ? launch_persistent<32, 7, true>(a, p, stream) : launch_persistent<32, 8, false>(a, p, stream); break;
-    }
-    if (rc != MIVOS_OK || p.splits == 1) return rc;
-    // split-K second pass: one thread per (row, 4 channels)
-    const int64_t work = p.rows * (a->cout_pad / 4);
-    int64_t grid = (work + 255) / 256;
-    if (grid > 148ll * 32) grid = 148ll * 32;
-    launch_pdl(splitk_epilogue_kernel, static_cast<unsigned>(grid), 256, 0, stream, p, bn);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    MIVOS_CUDA_OK(cudaGetLastError());
-    return MIVOS_OK;
-  }
-  CUtensorMap tmA, tmB;
-  int rc = encode_tmap_2d(&tmA, a->in, static_cast<uint64_t>(a->in_rows), static_cast<uint64_t>(a->in_cstride),
-                          static_cast<uint64_t>(a->in_cstride), 32, BM);
-  if (rc != MIVOS_OK) return rc;
-  rc = encode_tmap_2d(&tmB, a->weight, static_cast<uint64_t>(a->taps) * a->cout_pad, static_cast<uint64_t>(a->cin_pad),
-                      static_cast<uint64_t>(a->cin_pad), 32, static_cast<uint32_t>(bn));
-  if (rc != MIVOS_OK) return rc;
+  int rc = MIVOS_OK;
   switch (bn) {
-    case 256: return launch<256, 4>(a, tmA, tmB, p, stream);
-    case 128: return launch<128, 6>(a, tmA, tmB, p, stream);
-    case 64:  return launch<64, 8>(a, tmA, tmB, p, stream);
-    default:  return launch<32, 8>(a, tmA, tmB, p, stream);
+    // stage counts: a ring of ~190 KB of 128-byte k-block stages (one CTA per SM)
+    case 256: rc = a->in_f16 ? launch<256, 4, true>(a, p, stream) : launch<256, 4, false>(a, p, stream); break;
+    case 128: rc = a->in_f16 ? launch<128, 6, true>(a, p, stream) : launch<128, 6, false>(a, p, stream); break;
+    case 64:  rc = a->in_f16 ? launch<64, 8, true>(a, p, stream) : launch<64, 8, false>(a, p, stream); break;
+    default:  rc = a->in_f16 ? launch<32, 9, true>(a, p, stream) : launch<32, 9, false>(a, p, stream); break;
   }
+  if (rc != MIVOS_OK || p.splits == 1) return rc;
+  // split-K second pass: one thread per (row, 4 channels)
+  const int64_t work = p.rows * (a->cout_pad / 4);
+  int64_t grid = (work + 255) / 256;
+  if (grid > num_sms() * 32ll) grid = num_sms() * 32ll;
+  MIVOS_CUDA_OK(launch_pdl(splitk_epilogue_kernel, static_cast<unsigned>(grid), 256, 0, stream, p, bn));
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return MIVOS_OK;
 }

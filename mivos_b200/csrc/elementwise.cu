@@ -366,8 +366,8 @@ __global__ void copy_segments_kernel(const int64_t* __restrict__ fixed, const in
 }
 
 inline unsigned capped_grid(int64_t work) {
-  // grid-stride kernels: a few waves of 148 SMs x 8 resident 256-thread CTAs is plenty
-  const int64_t cap = 148ll * 16;
+  // grid-stride kernels: a few waves of the SMs x 8 resident 256-thread CTAs is plenty
+  const int64_t cap = num_sms() * 16ll;
   int64_t g = (work + kThreads - 1) / kThreads;
   if (g > cap) g = cap;
   if (g < 1) g = 1;

@@ -22,7 +22,7 @@ constexpr int kThreads = 256;
   } while (0)
 
 inline unsigned capped_grid(int64_t work) {
-  const int64_t cap = 148ll * 16;
+  const int64_t cap = num_sms() * 16ll;
   int64_t g = (work + kThreads - 1) / kThreads;
   if (g > cap) g = cap;
   if (g < 1) g = 1;

@@ -69,7 +69,7 @@ int num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;  // H100 SXM (no device visible: host-side planning only)
   }
   return n;
 }
@@ -104,8 +104,8 @@ extern "C" MIVOS_API int mivos_check_device(void) {
   MIVOS_CUDA_OK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   MIVOS_CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
-    set_last_error("mivos_b200 needs an sm_100 (B200) device; device %d is sm_%d%d — there is no fallback path",
+  if (prop.major != 9 || prop.minor != 0) {
+    set_last_error("mivos_b200 needs an sm_90 (H100) device; device %d is sm_%d%d — there is no fallback path",
                    dev, prop.major, prop.minor);
     return MIVOS_ERR_DEVICE;
   }

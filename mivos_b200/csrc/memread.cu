@@ -7,7 +7,7 @@
 //      (object, query, split) produces a short list of (score, slot) candidates:
 //        A1 `memread_exact_kernel`  : fp32 FMA scores on CUDA cores, exact per-split top-k
 //                                     (this file; also the overflow fallback of A2)
-//        A2 `memread_tc_kernel`     : TF32 tcgen05 scores + conservative threshold with an error
+//        A2 `memread_tc_kernel`     : TF32 wgmma scores + conservative threshold with an error
 //                                     margin (memread_tc.cu); survivors are re-scored exactly in B
 //   B. `memread_select_kernel`: per (object, query) merge candidates, (re-score,) exact top-k with
 //      a total order (score desc, slot asc), softmax over the k survivors
@@ -42,10 +42,11 @@ MemreadPlan memread_plan(int k_objects, int64_t slots, int hw, int top_k, int al
   }
   pl.qtiles = ceil_div(hw, pl.qtile);
   const int64_t tiles = ceil_div64(slots, pl.slot_tile);
-  // exact path: ~2 CTAs per SM; tcgen05 path: ONE wave of 148 CTAs (192 KB smem = 1 CTA/SM);
+  // exact path: ~2 CTAs per SM; tensor-core path: ONE wave of CTAs (~200 KB smem = 1 CTA/SM);
   // every split owns at least 4 slot tiles
-  int64_t want = algo == MIVOS_MEMREAD_TCGEN05 ? 148 / (static_cast<int64_t>(pl.qtiles) * k_objects)
-                                               : ceil_div64(296, static_cast<int64_t>(pl.qtiles) * k_objects);
+  const int64_t sms = num_sms();
+  int64_t want = algo == MIVOS_MEMREAD_TCGEN05 ? sms / (static_cast<int64_t>(pl.qtiles) * k_objects)
+                                               : ceil_div64(2 * sms, static_cast<int64_t>(pl.qtiles) * k_objects);
   int64_t max_by_tiles = tiles / 4 > 0 ? tiles / 4 : 1;
   int64_t s = want < max_by_tiles ? want : max_by_tiles;
   if (s < 1) s = 1;
@@ -640,7 +641,7 @@ extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* ban
   return MIVOS_ERR_INVALID;
 }
 
-// Debug/diagnostic (synchronises): candidate statistics of the last tcgen05-path read that used
+// Debug/diagnostic (synchronises): candidate statistics of the last tensor-core-path read that used
 // `workspace`: out[0] = total candidates after compaction, out[1] = max per (object, query),
 // out[2] = queries flagged for the exact fallback, out[3] = splits.
 extern "C" MIVOS_API int mivos_memory_read_stats(const void* workspace, int k_objects, int64_t slots, int hw,

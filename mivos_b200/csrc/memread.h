@@ -8,14 +8,14 @@ namespace mivos {
 
 constexpr int kMaxSplits = 16;
 constexpr int kMaxObjects = 256;  // objects (x lock-step clips) one memory-read call may serve
-constexpr int kTcCandCap = 512;   // candidates one (query, split) may hold while streaming (tcgen05 path)
+constexpr int kTcCandCap = 512;   // candidates one (query, split) may hold while streaming (tensor-core path)
 // A list ends at most kTcCandCap - 128 long (the streaming invariant: it is compacted against the current threshold
 // whenever it passes that, and flagged for the exact fallback if that does not help).  There is no further per-list
-// cap at the end of the kernel — a fixed 224 until the cfg-3 bench line (r02c12): with top-k 50 about 5 % of the
+// cap at the end of the kernel — with a fixed cap of 224 and top-k 50 about 5 % of the
 // queries ended above it, and ONE flagged query costs the exact fallback a whole 32-query tile over every slot
 // (5.1 ms per read).  The decision now belongs to the selection stage (pass A), which sees all lists of a query.
 constexpr int kSelMaxSurvivors = 1024;   // candidates (staged) / survivors (re-scored) the selection stage holds per query
-constexpr int kTcHalves = 2;      // column halves of a slot tile, one epilogue warpgroup (and list) each
+constexpr int kTcHalves = 2;      // column halves of a slot tile, one thread (and list) per query each
 constexpr int kMaxLists = kMaxSplits * kTcHalves;  // candidate lists per (object, query)
 // margin = 2*eps, eps = 1.05 * 2^-9 * ||q/sqrt(128)|| * max||key||  (see memread_tc.cu)
 constexpr float kTcMarginFactor = 2.0f * 1.05f * 0.001953125f;
@@ -26,7 +26,7 @@ struct MemreadPlan {
   int slot_tile;  // bank slots per inner tile
   int qtiles;
   int splits;  // CTAs along the memory axis
-  int nlists;  // candidate lists per (object, query): splits (exact) or splits * kTcHalves (tcgen05)
+  int nlists;  // candidate lists per (object, query): splits (exact) or splits * kTcHalves (tensor cores)
   int tiles_per_split;
   int kcap;  // list capacity per (object, query, split)
   // candidate lists are int2 {score bits, slot}: one 8-byte store per append, one load per read
@@ -35,7 +35,7 @@ struct MemreadPlan {
 
 MemreadPlan memread_plan(int k_objects, int64_t slots, int hw, int top_k, int algo);
 
-// First candidate list of a plan inside its workspace.  The tcgen05 plan's lists (kTcCandCap * 8 = 4096 bytes
+// First candidate list of a plan inside its workspace.  The tensor-core plan's lists (kTcCandCap * 8 = 4096 bytes
 // each) start on a 4 KB boundary, so no list straddles a 4 GB boundary and the generator bumps only the low
 // word of its append pointer (the plan reserves the 4 KB of slack).
 inline uint8_t* plan_lists(void* ws, const MemreadPlan& pl) {
@@ -48,7 +48,7 @@ inline uint8_t* plan_lists(void* ws, const MemreadPlan& pl) {
 int launch_exact_candidates(const float* bank_k, int64_t slots_cap, int k_objects, int64_t slots,
                             const float* qk, int hw, int q_div, int top_k, const MemreadPlan& pl, void* ws,
                             const int* flags, const int* dyn_slots, cudaStream_t stream);
-// Lists come from `pl`/`ws` (approximate scores that need the exact re-score when pl.algo is the tcgen05 plan).
+// Lists come from `pl`/`ws` (approximate scores that need the exact re-score when pl.algo is the tensor-core plan).
 // `flags` (optional, [K*hw]) and `pass`: pass 0 serves the queries whose flag is clear and SETS the flag of a query
 // whose lists hold more in-band candidates than the stage can stage (instead of selecting it); pass 1 serves only
 // the flagged queries (from the exact lists of the fallback).  flags == nullptr: one pass over every query.

@@ -1,14 +1,15 @@
-// Stage A2 of the memory read: candidate generation on the 5th-gen tensor cores.
+// Stage A2 of the memory read: candidate generation on the Hopper tensor cores.
 //
 // For one (object, 128-query tile, split of the memory axis) a CTA streams key tiles of 256 bank
 // slots through TMA (128B swizzle) and computes the affinity tile
 //     S[q, slot] = sum_c (qk[q,c]/sqrt(128)) * key[slot,c]
-// with tcgen05.mma kind::tf32 (M=128 queries, N=256 slots, K=8 per instruction, 16 instructions
-// per tile) into a double-buffered TMEM accumulator (2 x 256 columns).  The query operand stays
-// resident in shared memory (64 KB); keys flow through a 4-stage ring (4 x 32 KB).
+// with wgmma tf32 (two warpgroups of 64 queries each, N = 256 slots, K = 8 per instruction, 16
+// instructions per tile) into register accumulators.  The query operand stays resident in shared
+// memory (64 KB); keys flow through a 2-stage ring (2 x 32 KB) filled by one producer thread.
 //
-// Epilogue (2 x 4 warps — one warpgroup per column half of the slot tile —, one query per thread =
-// one TMEM lane): the thread streams its half of the row with tcgen05.ld and keeps
+// Epilogue (in each warpgroup: two threads per query, one per column half of the slot tile): the
+// accumulator fragment is transposed through a shared-memory tile, 64 columns per thread at a
+// time, and each thread keeps
 //   * NB "bucket maxima" in registers: NB values that are each a distinct score seen so far, so
 //     the top_k-th largest of them (tau) is a LOWER bound of the top_k-th largest score of the
 //     whole split.  (sorting them in place keeps the invariant; they are only ever max-updated.)
@@ -29,11 +30,10 @@
 // are served by the exact CUDA-core path (memread_exact_kernel + selection pass B), so adversarial
 // inputs (all-equal keys, huge-norm keys) stay correct.
 //
-// Roofline: tensor pipe.  Algorithmic flops 2*128*slots*hw per object; one 128x256x128 tile =
-// 16 MMAs x 128 cycles = 2048 cycles/SM at the TF32 rate.
+// Roofline: tensor pipe.  Algorithmic flops 2*128*slots*hw per object.
 #include "pdl.cuh"
 #include "memread.h"
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 #include <atomic>
 #include <cstdlib>
@@ -46,12 +46,12 @@ constexpr int TQ = 128;
 constexpr int TS = 256;
 constexpr int KB = 32;
 constexpr int NKB = 4;
-constexpr int STAGES = 4;
+constexpr int STAGES = 2;
 constexpr int QBLK_BYTES = TQ * KB * 4;       // 16 KB per k-block of the query tile
 constexpr int Q_BYTES = QBLK_BYTES * NKB;     // 64 KB
 constexpr int STAGE_BYTES = TS * KB * 4;      // 32 KB
 constexpr int WARM = 2;
-constexpr int TC_THREADS = 64 + 128 * kTcHalves;  // TMA warp, MMA warp, 2 epilogue warpgroups
+constexpr int TC_THREADS = 288;              // 2 MMA / epilogue warpgroups, TMA producer warp
 constexpr int STREAM_CAP = kTcCandCap;        // per (object, query, split) while streaming
 constexpr float kSqrtCK = 11.313708498984761f;
 constexpr float kEpsFactor = kTcMarginFactor;
@@ -194,7 +194,7 @@ __device__ __forceinline__ int compact_list(int2* list, int cnt, float thr) {
 // Append {score bits, slot} to the thread's list if the score passes.  Written in PTX so that it stays what it says:
 // one compare, one predicated 8-byte store, one predicated 64-bit bump.  (The C++ form of the same statement was
 // compiled into a 32-element prefix sum over materialised predicates with the addresses rebuilt per element:
-// ~15 instructions per tested score, ncu r02c4 source page; the epilogue is what bounds this kernel.)
+// ~15 instructions per tested score; the epilogue is what bounds this kernel.)
 // `lo` / `hi` are the halves of the append address: a list never straddles a 4 GB boundary (plan_lists), so only
 // the low word moves.
 __device__ __forceinline__ void emit_if_ge(int2*& lp, float v, float tau, int slot) {
@@ -213,6 +213,15 @@ __device__ __forceinline__ void emit_if_ge(int2*& lp, float v, float tau, int sl
       : "memory");
 }
 
+// Query rows of a warpgroup's 64 x 128 staging tile: columns [0, 64) of the chunk for half 0, [64, 128) for half 1;
+// the pad makes the fragment stores (8-byte pieces of 4 rows per half-warp) conflict-free.
+constexpr int STG_STRIDE = 136;
+constexpr int STG_BYTES = 64 * STG_STRIDE * 4;
+
+// Register budget: 168 per thread.  An SM's register file is split over its four scheduler partitions (16384
+// each); 9 warps put 3 on one partition, so 16384 / (3 x 32) caps a thread at 168 — a larger cap compiles but the
+// launch is refused.  The 128-float accumulator fragment, the NB bucket maxima and a 32-score chunk do not all fit
+// there: ptxas spills 0.3-1.3 KB per thread (NB = 32 / 64), served from L1, inside the candidate loop.
 template <int NB, bool EMIT_PTX>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -223,14 +232,12 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_q = smem;
   uint8_t* smem_k = smem + Q_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Q_BYTES + STAGES * STAGE_BYTES);
+  float* stg_all = reinterpret_cast<float*>(smem + Q_BYTES + STAGES * STAGE_BYTES);  // [2 warpgroups][64][STG_STRIDE]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Q_BYTES + STAGES * STAGE_BYTES + 2 * STG_BYTES);
   uint64_t* q_full = bars;
   uint64_t* full_bar = bars + 1;
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;       // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* tau_x = reinterpret_cast<float*>(tmem_slot + 2);  // [2][kTcHalves][128] thresholds exchanged between the halves
+  float* tau_x = reinterpret_cast<float*>(empty_bar + STAGES);  // [2][kTcHalves][128] thresholds exchanged between the halves
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * TQ;
@@ -246,42 +253,40 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   int t_end = t_begin + tps;
   if (t_end > total_tiles) t_end = total_tiles;
   const int nloc = t_end - t_begin;
+  // MMA / epilogue warpgroups 0 and 1 (warps 0-7): queries [0, 64) and [64, 128) of the tile; in each, warps 0-1 own
+  // the column half [0, 128) of every slot tile and warps 2-3 the half [128, 256), one query per thread.  Warp 8 is
+  // the TMA producer (see the register budget above the kernel)
+  const int wg = warp / 4;
+  const int tw = threadIdx.x & 127;
+  const int half = tw >> 6;
+  const int qi = wg * 64 + (tw & 63);  // query of this thread within the tile
   if (nloc <= 0) {
-    if (warp >= 2) {
-      const int qq = q0 + (warp & 3) * 32 + lane;
-      if (qq < p.hw)
-        p.cand_cnt[(static_cast<int64_t>(obj) * p.hw + qq) * p.nlists + split * kTcHalves + ((warp - 2) >> 2)] = 0;
+    if (warp < 8) {
+      const int qq = q0 + qi;
+      if (qq < p.hw) p.cand_cnt[(static_cast<int64_t>(obj) * p.hw + qq) * p.nlists + split * kTcHalves + half] = 0;
     }
     return;
   }
   const int warm = nloc < WARM ? nloc : WARM;
   const int nseq = nloc + warm;
 
-  if (warp == 0 && lane == 0) {
-    tc05::prefetch_tmap(&tmQ);
-    tc05::prefetch_tmap(&tmK);
-    tc05::mbar_init(q_full, 1);
+  if (threadIdx.x == 0) {
+    sm90::prefetch_tmap(&tmQ);
+    sm90::prefetch_tmap(&tmK);
+    sm90::mbar_init(q_full, 1);
     for (int s = 0; s < STAGES; ++s) {
-      tc05::mbar_init(&full_bar[s], 1);
-      tc05::mbar_init(&empty_bar[s], 1);
+      sm90::mbar_init(&full_bar[s], 1);
+      sm90::mbar_init(&empty_bar[s], 8);  // one arrival per MMA warp
     }
-    for (int b = 0; b < 2; ++b) {
-      tc05::mbar_init(&tmem_full[b], 1);
-      tc05::mbar_init(&tmem_empty[b], 4 * kTcHalves);  // one arrival per epilogue warp
-    }
-    tc05::fence_barrier_init();
+    sm90::fence_barrier_init();
   }
-  if (warp == 1) tc05::tmem_alloc<512>(tmem_slot);
-  tc05::fence_before_sync();
   __syncthreads();
-  tc05::fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (tc05::elect_one()) {
-      tc05::mbar_arrive_expect_tx(q_full, Q_BYTES);
+  if (warp == 8) {
+    if (lane == 0) {
+      sm90::mbar_arrive_expect_tx(q_full, Q_BYTES);
       // (the last tile of a set may run into the next set's rows: those lanes are masked by `valid`)
-      for (int kb = 0; kb < NKB; ++kb) tc05::tma_load_2d(smem_q + kb * QBLK_BYTES, &tmQ, q_full, kb * KB, qrow0 + q0);
+      for (int kb = 0; kb < NKB; ++kb) sm90::tma_load_2d(smem_q + kb * QBLK_BYTES, &tmQ, q_full, kb * KB, qrow0 + q0);
       const int64_t row0 = static_cast<int64_t>(obj) * p.slots_cap;
       int it = 0;
       for (int i = 0; i < nseq; ++i) {
@@ -290,229 +295,178 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         for (int kb = 0; kb < NKB; ++kb, ++it) {
           const int s = it % STAGES;
           const uint32_t ph = (it / STAGES) & 1;
-          if (p.spin_ns) tc05::mbar_wait_backoff(&empty_bar[s], ph ^ 1, p.err, 301, p.spin_ns);
-          else tc05::mbar_wait(&empty_bar[s], ph ^ 1, p.err, 301);
-          tc05::mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
-          tc05::tma_load_2d(smem_k + s * STAGE_BYTES, &tmK, &full_bar[s], kb * KB, row);
+          if (p.spin_ns) sm90::mbar_wait_backoff(&empty_bar[s], ph ^ 1, p.err, 301, p.spin_ns);
+          else sm90::mbar_wait(&empty_bar[s], ph ^ 1, p.err, 301);
+          sm90::mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
+          sm90::tma_load_2d(smem_k + s * STAGE_BYTES, &tmK, &full_bar[s], kb * KB, row);
         }
       }
     }
-  } else if (warp == 1) {
-    if (tc05::elect_one()) {
-      constexpr uint32_t idesc = tc05::make_idesc_tf32(TQ, TS);
-      tc05::mbar_wait(q_full, 0, p.err, 302);
-      const uint32_t q_addr = tc05::smem_u32(smem_q);
-      int it = 0;
-      for (int i = 0; i < nseq; ++i) {
-        const int buf = i & 1;
-        const uint32_t use = static_cast<uint32_t>(i >> 1);
-        if (p.spin_ns) tc05::mbar_wait_backoff(&tmem_empty[buf], (use & 1) ^ 1, p.err, 303, p.spin_ns);
-        else tc05::mbar_wait(&tmem_empty[buf], (use & 1) ^ 1, p.err, 303);
-        tc05::fence_after_sync();
-        const uint32_t d = tmem_base + buf * TS;
-        for (int kb = 0; kb < NKB; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          if (p.spin_ns) tc05::mbar_wait_backoff(&full_bar[s], ph, p.err, 304, p.spin_ns);
-          else tc05::mbar_wait(&full_bar[s], ph, p.err, 304);
-          tc05::fence_after_sync();
-          const uint64_t da = tc05::make_desc_sw128(q_addr + kb * QBLK_BYTES);
-          const uint64_t db = tc05::make_desc_sw128(tc05::smem_u32(smem_k + s * STAGE_BYTES));
-#pragma unroll
-          for (int k = 0; k < KB / 8; ++k)
-            tc05::umma_tf32_ss(d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          tc05::umma_commit(&empty_bar[s]);
-        }
-        tc05::umma_commit(&tmem_full[buf]);
-      }
-    }
-  } else {
-    // ------------------------------------------------------- epilogue: warps 2..5 own columns
-    // [0,128) of every slot tile, warps 6..9 columns [128,256); each keeps its own list
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int q = q0 + quarter * 32 + lane;
-    const bool valid = q < p.hw;
-    const int64_t lq = static_cast<int64_t>(obj) * p.hw + (valid ? q : 0);
-    const float margin = valid ? kEpsFactor * p.qnorm[qrow0 + q] * sqrtf(p.kmax2[obj]) : 0.f;
-    const int64_t list_id = lq * p.nlists + split * kTcHalves + half;
-    int2* const list = p.cand + list_id * STREAM_CAP;
-    int2* lp = list;  // append pointer (count = lp - list)
-    float m[NB];
-#pragma unroll
-    for (int b = 0; b < NB; ++b) m[b] = -INFINITY;
-    float tau_emit = -INFINITY;
-    bool overflow = false;
-    int retau_n = 0;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-
-    for (int i = 0; i < nseq; ++i) {
-      const int buf = i & 1;
-      const uint32_t use = static_cast<uint32_t>(i >> 1);
-      tc05::mbar_wait(&tmem_full[buf], use & 1, p.err, 305);
-      tc05::fence_after_sync();
-      const int tile = t_begin + (i < nloc ? i : i - nloc);
-      const int64_t slot0 = static_cast<int64_t>(tile) * TS;
-      const int64_t rem = slots - slot0;
-      const int ncols = rem < TS ? static_cast<int>(rem) : TS;
-      const bool emit = (i >= warm) && valid && !overflow;
-      if constexpr (NB == 32) {
-        // The row is read 16 columns at a time and the TMEM read of the next 16 is issued before the current 16 are
-        // processed (two 16-register sets): the first use of a freshly loaded chunk was where this warp waited
-        // (long-scoreboard stalls on the first FMNMX after every tcgen05.ld, 20 % of the kernel's samples on real
-        // data, profiles/r02c12_ncu_memread_real_4clips.txt).
-        constexpr int SPH = TS / 16 / kTcHalves;  // sub-chunks of 16 columns per half
-        uint32_t vra[16], vrb[16];
-        const uint32_t tbase = lane_addr + buf * TS + half * (TS / kTcHalves);
-        tc05::tmem_ld16(tbase, vra);
-  #pragma unroll
-        for (int sc = 0; sc < SPH; ++sc) {
-          tc05::tmem_ld_wait();
-          if (sc + 1 < SPH) tc05::tmem_ld16(tbase + (sc + 1) * 16, (sc & 1) ? vra : vrb);
-          const int col0 = half * (TS / kTcHalves) + sc * 16;
-          float v[16];
-  #pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __uint_as_float((sc & 1) ? vrb[j] : vra[j]);
-          if (col0 + 16 > ncols) {
-  #pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (col0 + j >= ncols) v[j] = -INFINITY;  // stale rows past the live bank
-          }
-          // bucket maxima (bucket = column mod NB).  NOT on the replayed warm tiles: m[] is sorted in place between
-          // tiles, so re-presenting an element already witnessed could store it in a second position and
-          // break the "NB distinct scores" invariant that makes tau a lower bound.
-          if (i < nloc) {
-            const int b0 = ((NB == 64 && ((sc >> 1) & 1)) ? 32 : 0) + (sc & 1) * 16;  // a constant once unrolled
-  #pragma unroll
-            for (int j = 0; j < 16; ++j) m[b0 + j] = fmaxf(m[b0 + j], v[j]);
-          }
-          if (emit) {
-            const int idx0 = static_cast<int>(slot0) + col0;
-            if constexpr (EMIT_PTX) {
-  #pragma unroll
-              for (int j = 0; j < 16; ++j) emit_if_ge(lp, v[j], tau_emit, idx0 + j);
-            } else {
-  #pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const bool pass = v[j] >= tau_emit;
-                if (pass) *lp = make_int2(__float_as_int(v[j]), idx0 + j);
-                lp += pass ? 1 : 0;
-              }
-            }
-          }
-        }
-      } else {
-        // NB = 64 (top-k > 32): 32 columns per tcgen05.ld, consumed before the next read is issued.  The pipelined
-        // form above measured SLOWER here (cfg-5, where nothing else differed between the two runs: memory read
-        // 6.40 -> 6.89 ms, profiles/r02c13_bench_cfg5.json vs r02c14_bench_cfg5.json; 168 registers either way).
-#pragma unroll 2
-        for (int c = half * (TS / 32 / kTcHalves); c < (half + 1) * (TS / 32 / kTcHalves); ++c) {
-          uint32_t vr[32];
-          tc05::tmem_ld32(lane_addr + buf * TS + c * 32, vr);
-          tc05::tmem_ld_wait();
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(vr[j]);
-          if (c * 32 + 32 > ncols) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c * 32 + j >= ncols) v[j] = -INFINITY;  // stale rows past the live bank
-          }
-          if (i < nloc) {  // (see the note on the replayed tiles above)
-            if (c & 1) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) m[(32 + j) % NB] = fmaxf(m[(32 + j) % NB], v[j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) m[j] = fmaxf(m[j], v[j]);
-            }
-          }
-          if (emit) {
-            const int idx0 = static_cast<int>(slot0) + c * 32;
-            if constexpr (EMIT_PTX) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) emit_if_ge(lp, v[j], tau_emit, idx0 + j);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const bool pass = v[j] >= tau_emit;
-                if (pass) *lp = make_int2(__float_as_int(v[j]), idx0 + j);
-                lp += pass ? 1 : 0;
-              }
-            }
-          }
-        }
-      }
-      tc05::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc05::mbar_arrive(&tmem_empty[buf]);
-
-      // threshold schedule: end of warm-up, then every 4th tile, and before the replay
-      const bool retau = (i + 1 == warm) || (i + 1 > warm && ((i + 1 - warm) & 3) == 0) || (i + 1 == nloc);
-      // clamp above -inf: masked (stale) columns carry -inf and must never pass `v >= tau_emit`
-      if (retau) {
-        // Any subset's k-th largest score is a lower bound of the global k-th largest, so the best
-        // bound found by ANY CTA working on this query (other splits, the other column half) is as
-        // valid as our own: share it through one atomicMax per refresh.  This is what keeps the
-        // lists short: without it every list keeps what beats ITS OWN k-th score (~2100 candidates
-        // per query at a 20-frame bank instead of a few hundred).  Which bound is visible when is a
-        // matter of timing, so list lengths vary from run to run; the selected top-k does not.
-        // A second, tighter bound from the PAIR of column halves: they saw disjoint slots, so if this half holds
-        // ceil(k/2) distinct scores >= a and the other ceil(k/2) distinct scores >= b, the two together hold k
-        // scores >= min(a, b).  (k-th of 64 bucket maxima at k = 50 is a weak bound — 1.5 x bucket-size scores
-        // pass it; the 25th of 64 in each half lets a third of that through.  CPU model on cfg-3 features:
-        // scores within the final threshold 930 -> 380 per query; the in-band minimum is 117.)
-        float t, t_half;
-        kth_pair<NB>(m, p.top_k, (p.top_k + 1) >> 1, t, t_half);
-        {
-          float* tx = tau_x + (retau_n & 1) * (kTcHalves * 128);  // two buffers: one barrier per exchange
-          ++retau_n;
-          tx[half * 128 + quarter * 32 + lane] = t_half;
-          asm volatile("bar.sync 1, %0;" ::"n"(128 * kTcHalves) : "memory");
-          float pair = t_half;
-#pragma unroll
-          for (int hh = 0; hh < kTcHalves; ++hh) pair = fminf(pair, tx[hh * 128 + quarter * 32 + lane]);
-          t = fmaxf(t, pair);
-        }
-        if (valid) {
-          const int enc = float_ordered(fmaxf(t, -3.0e38f));
-          const int prev = atomicMax(p.tau_g + lq, enc);
-          t = ordered_float(prev > enc ? prev : enc);
-        }
-        tau_emit = fmaxf(t - margin, -3.0e38f);
-      }
-      // keep room for this warpgroup's share of a full tile of appends
-      if ((lp - list) > STREAM_CAP - TS / kTcHalves && !overflow) {
-        const int kept = compact_list(list, static_cast<int>(lp - list), tau_emit);
-        lp = list + kept;
-        if (kept > STREAM_CAP - TS / kTcHalves) overflow = true;
-      }
-    }
-    // Final threshold: both column halves saw disjoint parts of the same split, each tau is a
-    // lower bound of the split's k-th largest score, hence so is their maximum.
-    // (the last refresh of the loop ran at i + 1 == nloc, before the replayed tiles, which do not touch m[]:
-    // tau_g already holds this CTA's final bounds, the pair bound included)
-    float tau_fin = kth_largest<NB>(m, p.top_k);
-    if (valid) tau_fin = fmaxf(tau_fin, ordered_float(__ldcg(p.tau_g + lq)));
-    if (valid) {
-      // Lists are left as they are: the selection stage filters them against the final shared threshold anyway, and
-      // it is the selection stage that sends a query whose lists carry more in-band candidates than it can hold to
-      // the exact CUDA-core path (memread.cu, pass A).  Only a list that overflowed while streaming flags here.
-      p.cand_cnt[list_id] = overflow ? 0 : static_cast<int>(lp - list);
-      if (overflow) atomicExch(p.overflow + lq, 1);
-    }
+    return;
   }
 
-  tc05::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc05::fence_after_sync();
-    tc05::tmem_dealloc<512>(tmem_base);
+  const uint32_t bar_id = 1 + wg;  // named barrier of this warpgroup
+  float* const stg = stg_all + wg * 64 * STG_STRIDE;
+  const int q = q0 + qi;
+  const bool valid = q < p.hw;
+  const int64_t lq = static_cast<int64_t>(obj) * p.hw + (valid ? q : 0);
+  const float margin = valid ? kEpsFactor * p.qnorm[qrow0 + q] * sqrtf(p.kmax2[obj]) : 0.f;
+  const int64_t list_id = lq * p.nlists + split * kTcHalves + half;
+  int2* const list = p.cand + list_id * STREAM_CAP;
+  int2* lp = list;  // append pointer (count = lp - list)
+  float m[NB];
+#pragma unroll
+  for (int b = 0; b < NB; ++b) m[b] = -INFINITY;
+  float tau_emit = -INFINITY;
+  bool overflow = false;
+  int retau_n = 0;
+  float acc[TS / 2];  // wgmma fragment of the 64 x 256 score tile
+  sm90::mbar_wait(&q_full[0], 0, p.err, 302);
+  const uint32_t q_addr = sm90::smem_u32(smem_q) + wg * 64 * 128;
+  // fragment coordinates of this thread: rows fr, fr + 8, columns 8j + fc, 8j + fc + 1
+  const int fr = (tw >> 5) * 16 + ((tw & 31) >> 2);
+  const int fc = 2 * (tw & 3);
+
+  int it = 0;
+  for (int i = 0; i < nseq; ++i) {
+    int prev = -1;
+    // (the first wgmma overwrites the fragment: zeroing it here tells the compiler that the previous tile's values
+    // are dead, so they do not occupy registers across the threshold refresh)
+#pragma unroll
+    for (int j = 0; j < TS / 2; ++j) acc[j] = 0.f;
+    for (int kb = 0; kb < NKB; ++kb, ++it) {
+      const int s = it % STAGES;
+      sm90::mbar_wait(&full_bar[s], (it / STAGES) & 1, p.err, 304);
+      const uint64_t da = sm90::make_desc_sw128(q_addr + kb * QBLK_BYTES);
+      const uint64_t db = sm90::make_desc_sw128(sm90::smem_u32(smem_k + s * STAGE_BYTES));
+      sm90::wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < KB / 8; ++k) sm90::wgmma<TS, false>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      sm90::wgmma_commit();
+      sm90::wgmma_wait<1>();  // the previous k-block's wgmmas are done: its stage may be refilled
+      if (prev >= 0 && lane == 0) sm90::mbar_arrive(&empty_bar[prev]);
+      prev = s;
+    }
+    sm90::wgmma_wait<0>();
+    sm90::fence_acc(acc);
+    if (lane == 0) sm90::mbar_arrive(&empty_bar[prev]);
+
+    const int tile = t_begin + (i < nloc ? i : i - nloc);
+    const int64_t slot0 = static_cast<int64_t>(tile) * TS;
+    const int64_t rem = slots - slot0;
+    const int ncols = rem < TS ? static_cast<int>(rem) : TS;
+    const bool emit = (i >= warm) && valid && !overflow;
+    // Two chunks: chunk c holds columns [64c, 64c + 64) of half 0 and [128 + 64c, ...) of half 1; the warpgroup parks
+    // them in its staging tile and every thread reads back the 64 scores of its own query and half, 32 at a time.
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      sm90::named_sync(bar_id, 128);  // the previous chunk has been read
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int j = h * 16 + 8 * c + jj;
+          float* dst = stg + fr * STG_STRIDE + h * 64 + 8 * jj + fc;
+          *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(dst + 8 * STG_STRIDE) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      sm90::named_sync(bar_id, 128);
+#pragma unroll
+      for (int sb = 0; sb < 2; ++sb) {
+        float v[32];
+        const float* src = stg + (tw & 63) * STG_STRIDE + half * 64 + sb * 32;
+#pragma unroll
+        for (int j = 0; j < 32; j += 4) {
+          const float4 t = *reinterpret_cast<const float4*>(src + j);
+          v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
+        }
+        const int col0 = half * (TS / kTcHalves) + c * 64 + sb * 32;  // tile column of v[0]
+        if (col0 + 32 > ncols) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j)
+            if (col0 + j >= ncols) v[j] = -INFINITY;  // stale rows past the live bank
+        }
+        // bucket maxima (bucket = column mod NB).  NOT on the replayed warm tiles: m[] is sorted in place between
+        // tiles, so re-presenting an element already witnessed could store it in a second position and break the
+        // "NB distinct scores" invariant that makes tau a lower bound.
+        if (i < nloc) {
+          const int off = (NB == 64 && sb) ? 32 : 0;  // a constant once unrolled
+#pragma unroll
+          for (int j = 0; j < 32; ++j) m[(off + j) % NB] = fmaxf(m[(off + j) % NB], v[j]);
+        }
+        if (emit) {
+          const int idx0 = static_cast<int>(slot0) + col0;
+          if constexpr (EMIT_PTX) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) emit_if_ge(lp, v[j], tau_emit, idx0 + j);
+          } else {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              const bool pass = v[j] >= tau_emit;
+              if (pass) *lp = make_int2(__float_as_int(v[j]), idx0 + j);
+              lp += pass ? 1 : 0;
+            }
+          }
+        }
+      }
+    }
+
+    // threshold schedule: end of warm-up, then every 4th tile, and before the replay
+    const bool retau = (i + 1 == warm) || (i + 1 > warm && ((i + 1 - warm) & 3) == 0) || (i + 1 == nloc);
+    // clamp above -inf: masked (stale) columns carry -inf and must never pass `v >= tau_emit`
+    if (retau) {
+      // Any subset's k-th largest score is a lower bound of the global k-th largest, so the best
+      // bound found by ANY CTA working on this query (other splits, the other column half) is as
+      // valid as our own: share it through one atomicMax per refresh.  This is what keeps the
+      // lists short: without it every list keeps what beats ITS OWN k-th score.  Which bound is
+      // visible when is a matter of timing, so list lengths vary from run to run; the selected
+      // top-k does not.
+      // A second, tighter bound from the PAIR of column halves: they saw disjoint slots, so if this half holds
+      // ceil(k/2) distinct scores >= a and the other ceil(k/2) distinct scores >= b, the two together hold k
+      // scores >= min(a, b).
+      float t, t_half;
+      kth_pair<NB>(m, p.top_k, (p.top_k + 1) >> 1, t, t_half);
+      {
+        float* tx = tau_x + (retau_n & 1) * (kTcHalves * 128);  // two buffers: one barrier per exchange
+        ++retau_n;
+        tx[half * 128 + qi] = t_half;
+        sm90::named_sync(bar_id, 128);  // both halves of a query are in this warpgroup
+        float pair = t_half;
+#pragma unroll
+        for (int hh = 0; hh < kTcHalves; ++hh) pair = fminf(pair, tx[hh * 128 + qi]);
+        t = fmaxf(t, pair);
+      }
+      if (valid) {
+        const int enc = float_ordered(fmaxf(t, -3.0e38f));
+        const int prev_t = atomicMax(p.tau_g + lq, enc);
+        t = ordered_float(prev_t > enc ? prev_t : enc);
+      }
+      tau_emit = fmaxf(t - margin, -3.0e38f);
+    }
+    // keep room for this thread's share of a full tile of appends
+    if ((lp - list) > STREAM_CAP - TS / kTcHalves && !overflow) {
+      const int kept = compact_list(list, static_cast<int>(lp - list), tau_emit);
+      lp = list + kept;
+      if (kept > STREAM_CAP - TS / kTcHalves) overflow = true;
+    }
+  }
+  // Final threshold: both column halves saw disjoint parts of the same split, each tau is a
+  // lower bound of the split's k-th largest score, hence so is their maximum.
+  // (the last refresh of the loop ran at i + 1 == nloc, before the replayed tiles, which do not touch m[]:
+  // tau_g already holds this CTA's final bounds, the pair bound included)
+  float tau_fin = kth_largest<NB>(m, p.top_k);
+  if (valid) tau_fin = fmaxf(tau_fin, ordered_float(__ldcg(p.tau_g + lq)));
+  if (valid) {
+    // Lists are left as they are: the selection stage filters them against the final shared threshold anyway, and
+    // it is the selection stage that sends a query whose lists carry more in-band candidates than it can hold to
+    // the exact CUDA-core path (memread.cu, pass A).  Only a list that overflowed while streaming flags here.
+    p.cand_cnt[list_id] = overflow ? 0 : static_cast<int>(lp - list);
+    if (overflow) atomicExch(p.overflow + lq, 1);
   }
 }
 
-constexpr int TC_SMEM = Q_BYTES + STAGES * STAGE_BYTES + 16 * 8 + 2 * 128 * kTcHalves * 4 + 1024;
+constexpr int TC_SMEM = Q_BYTES + STAGES * STAGE_BYTES + 2 * STG_BYTES + (1 + 2 * STAGES) * 8 + 2 * 128 * kTcHalves * 4 + 1024;
 
 }  // namespace
 
@@ -523,7 +477,7 @@ int memread_tc_run(const float* bank_k, const float* bank_v, int64_t slots_cap, 
                    int out_coff, int halo_h, int halo_w, int out_f16, int32_t* topk_idx, float* topk_val,
                    void* workspace, const int* dyn_slots, cudaStream_t stream) {
   MIVOS_REQUIRE(static_cast<int64_t>(k_objects) * slots_cap < (1ll << 31) - 4096,
-                "memory_read(tcgen05): bank rows exceed int32 TMA coordinates");
+                "memory_read(tensor cores): bank rows exceed int32 TMA coordinates");
   const MemreadPlan tc = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_TCGEN05);
   const MemreadPlan ex = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
   uint8_t* w = static_cast<uint8_t*>(workspace);
@@ -575,8 +529,8 @@ int memread_tc_run(const float* bank_k, const float* bank_v, int64_t slots_cap, 
   p.tau_g = tau_g;
   p.err = device_error_flag();
 
-  // A/B switches (measured on B200, profiles/r02c10_*): MIVOS_MEMREAD_EMIT=c restores the compiler's emission
-  // loop, MIVOS_MEMREAD_BACKOFF_NS=0 the flat-out barrier polls
+  // MIVOS_MEMREAD_EMIT=c selects the compiler's emission loop, MIVOS_MEMREAD_BACKOFF_NS the producer's sleep
+  // between barrier polls (0 = poll flat out)
   static const bool emit_ptx = [] { const char* e = getenv("MIVOS_MEMREAD_EMIT"); return !(e && e[0] == 'c'); }();
   static const unsigned spin_ns = [] { const char* e = getenv("MIVOS_MEMREAD_BACKOFF_NS"); return e ? static_cast<unsigned>(atoi(e)) : 100u; }();
   p.spin_ns = spin_ns;
@@ -600,7 +554,7 @@ int memread_tc_run(const float* bank_k, const float* bank_v, int64_t slots_cap, 
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 
-  // selection pass A: every query the candidate pass did not flag, from the tcgen05 lists; a query whose lists carry
+  // selection pass A: every query the candidate pass did not flag, from the tensor-core lists; a query whose lists carry
   // more in-band candidates than the stage can hold is flagged there instead of being selected
   rc = launch_select(bank_k, bank_v, slots_cap, k_objects, qk, hw, q_div, top_k, tc, w_tc, nullptr, nullptr, flags, 0, qnorm,
                      reinterpret_cast<const float*>(kmax2), tau_g, out, out_cstride, out_coff, halo_h, halo_w, out_f16, topk_idx,

@@ -4,7 +4,7 @@
 // cudaLaunchAttributeProgrammaticStreamSerialization and
 //   * executes griddepcontrol.launch_dependents first, so the NEXT kernel's CTAs are scheduled as
 //     soon as this grid's CTAs have all started and SMs free up, and run their prologue
-//     (barrier init, TMEM allocation, tensor-map prefetch) under this grid's tail;
+//     (barrier init, tensor-map prefetch) under this grid's tail;
 //   * executes griddepcontrol.wait before its first access to global memory, which blocks until
 //     the PREVIOUS grid has completed and its writes are visible — so the data dependences (and
 //     the write-after-read ones) of plain stream order are kept.

@@ -300,7 +300,7 @@ class PropagationEngine(_ResNetTrunk):
         """get_query_values (prop_net.py:164-168) + the decoder skip paths for N frames at once
         (`frames` [N,3,H,W] on the device, `batch` the batched QueryState from new_query_states).
         Batching multiplies the tile count of the 1/8- and 1/16-resolution layers by N, which is
-        what fills the 148 SMs."""
+        what fills the 132 SMs."""
         N, _, H, W = frames.shape
         assert H % 16 == 0 and W % 16 == 0, "frames must be padded to multiples of 16 (pad_divide_by)"
         ws = self.ws_q
@@ -394,7 +394,7 @@ class PropagationEngine(_ResNetTrunk):
     # ------------------------------------------------------------------ lock-step multi-clip step
     # C independent clips advance one frame per call as ONE batch of C*K maps through every
     # convolution (row tiles per launch x C: the 1/16- and 1/8-resolution layers of a single clip
-    # have 14-54 row tiles for 148 SMs).  The operators whose operands differ per clip — the memory
+    # have 14-54 row tiles for 132 SMs).  The operators whose operands differ per clip — the memory
     # read (own bank, own query), the skip-path broadcast, the stem gather and the aggregation over a
     # clip's objects — take the C clips as groups of ONE launch (query sets / skip_n / groups of the C ABI).
     # Object maps are clip-major: image c*K + k is object k of clip c.
@@ -474,7 +474,7 @@ class S2MEngine(_ResNetTrunk):
     16 (model/s2m/s2m_network.py:8-33, s2m_resnet.py:70-148, _deeplab.py:30-58,119-160), for a batch of
     n inputs (one per object of an interaction: davis_processor.py:55-68, s2m_controller.py:28-35).
 
-    Every convolution is a tcgen05 implicit GEMM (mivos_conv_gemm); BatchNorm is folded at pack time;
+    Every convolution is a wgmma implicit GEMM (mivos_conv_gemm); BatchNorm is folded at pack time;
     the dilated 3x3 convs (layer4 blocks 1-2, the three ASPP branches) read a dilated gather; the
     image-pooling branch is pooled and broadcast BEFORE its 1x1 conv (the conv, BN and ReLU commute
     with broadcasting a constant map), so that its output lands straight in the 1280-channel concat

@@ -1,6 +1,6 @@
 """Drop-in ``FusionNet`` (reference: model/fusion_net.py:8-50): same constructor, state_dict keys
 (``conv1.0 conv2.{0,2} conv3.{0,2} final_conv``) and ``forward`` signature; the six full-resolution
-3x3 convolutions run as tcgen05 implicit GEMMs on a HALO (1,H,W,32) map."""
+3x3 convolutions run as wgmma implicit GEMMs on a HALO (1,H,W,32) map."""
 from __future__ import annotations
 
 from typing import Optional

@@ -136,7 +136,7 @@ class InferenceCore:
         self.mem_freq = mem_freq
 
         # Same buffer policy table as the reference (:44-63).  Results always live on the device
-        # here (B200 has 180 GB; a 480p prob volume is 1.66 MB per frame per object); the
+        # here (a 480p prob volume is 1.66 MB per frame per object); the
         # query-feature cache honours q_buf_size, image staging honours data_dev / i_buf_size.
         if mem_profile == 0:
             self.data_dev, self.q_buf_size, self.i_buf_size = self.device, 105, -1

@@ -3,7 +3,7 @@
 The reference propagates one sequence per process call (eval_interactive_davis.py:76-83 builds a
 fresh processor per sequence); sequences share nothing, which is what shards them over GPUs
 (SURVEY.md §8e).  The same independence can be used INSIDE a GPU: the per-frame chain of one clip
-is ~70 short dependent kernels whose 1/16- and 1/8-resolution layers have 14-54 row tiles for 148
+is ~70 short dependent kernels whose 1/16- and 1/8-resolution layers have 14-54 row tiles for 132
 SMs, so C clips that advance together — same clip length, same interaction history, hence the same
 ``schedule.PassPlan`` — go through every convolution as one batch of C*K maps (C times the tiles
 per launch, one launch instead of C), while the operators whose operands differ per clip (memory

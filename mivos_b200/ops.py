@@ -1,6 +1,6 @@
 """Thin torch-tensor wrappers over the C ABI (include/mivos_b200.h).
 
-PyTorch is used here only for device memory and streams; every op launches hand-written sm_100a
+PyTorch is used here only for device memory and streams; every op launches hand-written sm_90a
 kernels from ``libmivos_b200.so``.  Nothing in this module has a CPU or PyTorch fallback.
 
 Layouts (see the header): HALO = [N, H+2, W+2, C] with a zero border, fp32 (TF32 tensor-core path)

@@ -1,7 +1,7 @@
 """Drop-in ``PropagationNetwork`` (reference: model/propagation/prop_net.py:131-200).
 
 Same constructor, same ``state_dict`` keys (597 tensors), same public methods and tensor
-layouts at the boundary; every method runs hand-written sm_100a kernels through the C ABI.
+layouts at the boundary; every method runs hand-written sm_90a kernels through the C ABI.
 Internally features stay in the HALO layout; the reference-layout (NCHW) entry points convert at
 the boundary, while ``InferenceCore`` uses the ``*_resident`` methods that never leave HBM-native
 layouts.

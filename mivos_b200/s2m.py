@@ -9,7 +9,7 @@ Reference surface kept:
   * ``interact.s2m_controller.S2MController(s2m_net, num_objects, ignore_class, device)`` with
     ``interact(image, prev_mask, scr_mask) -> [K,1,nh,nw]`` (interact/s2m_controller.py:10-37)
 
-The network runs on the same tcgen05 implicit-GEMM convolution as the propagation path
+The network runs on the same wgmma implicit-GEMM convolution as the propagation path
 (engine.S2MEngine); there is no CPU or PyTorch path.
 """
 from __future__ import annotations

@@ -18,7 +18,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from oracle import refshim, stm_oracle as O, weights as Wt  # noqa: E402
+from oracle import golden_io, refshim, stm_oracle as O, weights as Wt  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 
@@ -95,7 +95,7 @@ def main():
     fu_orc = O.fusion_net(fsd, images[:, 3], seg_ref[0:1], agg_ref[1:2], at_ref, dist)
     _cmp("fusion", fu_orc, fu_ref, report)
     g.update(pos=_np(pos), neg=_np(neg), attn=_np(at_ref), fuse=_np(fu_ref), dist=_np(dist))
-    np.savez_compressed(os.path.join(OUT, "ops_lowres.npz"), **g)
+    golden_io.save(os.path.join(OUT, "ops_lowres.npz"), g)
 
     # ------------------------------------------------------------------ memory-read goldens (random tensors)
     gm = torch.Generator().manual_seed(5)
@@ -108,7 +108,7 @@ def main():
         o = torch.cat([O.memory_read(mk[i:i + 1], mv[i:i + 1], qk, k_) for i in range(2)], 0)
         _cmp(f"memread_top{k_}", o, r, report)
         rd[f"out{k_}"] = _np(r)
-    np.savez_compressed(os.path.join(OUT, "memread.npz"), mk=_np(mk), mv=_np(mv), qk=_np(qk), **rd)
+    golden_io.save(os.path.join(OUT, "memread.npz"), dict(mk=_np(mk), mv=_np(mv), qk=_np(qk), **rd))
 
     # ------------------------------------------------------------------ whole-clip golden, low res, with fusion
     T, h, w, K = 6, 64, 88, 2  # 88 -> padded to 96: exercises pad/unpad

@@ -34,7 +34,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from oracle import stm_oracle as O, weights as Wt  # noqa: E402
+from oracle import golden_io, stm_oracle as O, weights as Wt  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 
@@ -82,14 +82,14 @@ def run_case(name: str, psd, fsd) -> dict:
         out = core.interact(m, idx)
     dt = time.perf_counter() - t0
     last_ti = core.bank_trace[-1][0]
-    np.savez_compressed(
+    golden_io.save(
         os.path.join(OUT, f"full_{name}.npz"),
-        masks=out.astype(np.uint8),
-        prob_s=core.prob[:, :, 0, ::S, ::S].numpy().astype(np.float16),
-        prob_l=core.prob[:, last_ti, 0].numpy().astype(np.float16),
-        last_ti=np.int32(last_ti),
-        trace=np.asarray(core.bank_trace, dtype=np.int32),
-        stride=np.int32(S))
+        dict(masks=out.astype(np.uint8),
+             prob_s=core.prob[:, :, 0, ::S, ::S].numpy().astype(np.float16),
+             prob_l=core.prob[:, last_ti, 0].numpy().astype(np.float16),
+             last_ti=np.int32(last_ti),
+             trace=np.asarray(core.bank_trace, dtype=np.int32),
+             stride=np.int32(S)))
     frames = len(core.bank_trace)
     return {"frames_propagated": frames, "cpu_seconds": round(dt, 1), "cpu_fps": round(frames / dt, 3),
             "threads": torch.get_num_threads(), "mask_pixels_fg": int((out > 0).sum()),

@@ -4,7 +4,7 @@ over ``mivos_b200.ops`` by tests/test_s2m_cpu.py and tests/test_engine_cpu.py so
 the engines — weight packing, channel windows of the concat buffers, dilation tables, buffer shapes,
 gather orders, the decoder's skip/broadcast plumbing — can be checked against the reference-generated
 golden vectors without a GPU.  It says nothing
-about the kernels themselves (tests/test_gpu_z_s2m.py does, on a B200) and nothing in the product
+about the kernels themselves (tests/test_gpu_z_s2m.py does, on an H100) and nothing in the product
 package imports it."""
 from __future__ import annotations
 

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with `-m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with `-m gpu`)")
 
 
 @pytest.fixture(scope="session", autouse=True)
@@ -35,8 +35,10 @@ def fuse_sd():
 
 @pytest.fixture(scope="session")
 def golden():
+    from oracle import golden_io
+
     def load(name):
-        return np.load(os.path.join(GOLDEN, name))
+        return golden_io.load(os.path.join(GOLDEN, name))
     return load
 
 

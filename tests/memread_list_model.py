@@ -1,4 +1,4 @@
-"""CPU model of the candidate lists of the memory read's tcgen05 pass (mivos_b200/csrc/memread_tc.cu) — test
+"""CPU model of the candidate lists of the memory read's tensor-core pass (mivos_b200/csrc/memread_tc.cu) — test
 infrastructure, like the oracle it imports.  It replays the kernel's bookkeeping in numpy on real key / query
 features of the oracle network: streams = (split of the slot axis) x (column half of a 256-slot tile); per stream
 NB bucket maxima (bucket = column mod NB), thresholds refreshed after the warm-up tiles, every 4th tile and at the
@@ -12,8 +12,7 @@ Numbers this produced on the synthetic cfg-3 clip (seeded random weights; margin
   k-th-of-64 thresholds only : 1440-1730 candidates per query in the lists, 930 of them within the final threshold,
                                5 % of the queries above the old per-list cap of 224 -> 3/4 of the exact fallback's tiles
   + PAIR rule                : 380 within the final threshold (the in-band minimum is 117), none flagged
-which, with the fallback decision moved into the selection stage, moved the cfg-3 bench line from 140 to 438 frames/s
-(profiles/r02c12_*, r02c17_*)."""
+(the fallback decision moved into the selection stage)."""
 import math
 import sys
 
@@ -51,7 +50,7 @@ def run(mk, qk, top_k, pair, verbose=True):
     q = (qk.reshape(CK, hw).T / np.float32(math.sqrt(128))).astype(np.float32)
     NB, TS, CAP = (32 if top_k <= 32 else 64), 256, 512
     qtiles, tiles = (hw + 127) // 128, (slots + TS - 1) // TS
-    s = max(1, min(148 // (qtiles * Kk), max(1, tiles // 4), 16))
+    s = max(1, min(132 // (qtiles * Kk), max(1, tiles // 4), 16))  # one wave on the 132 SMs of an H100
     tps = (tiles + s - 1) // s
     splits = (tiles + tps - 1) // tps
     out = []

@@ -1,12 +1,19 @@
-"""CPU, build container only: UNCHANGED caller files of the reference, loaded straight from /root/reference,
+"""CPU: UNCHANGED caller files of the reference, loaded straight from the reference checkout (oracle/refshim.py),
 running on top of THIS repository's import-path shims (`model.propagation.prop_net`, `model.aggregate`,
 `model.s2m.s2m_network`, `util.tensor_util` resolve to mivos_b200) — the drop-in claim of SURVEY §8(b)
 exercised literally.  The networks run over the emulated C-ABI operators (tests/abi_emulator.py); the
-same callers run on the real kernels wherever a B200 and the reference tree are both present.
+same callers run on the real kernels wherever an H100 and the reference tree are both present.
 
   * generation/fusion_generator.py   FusionGenerator (second client of the propagation surface, §8f-1)
   * interact/s2m_controller.py       S2MController (per-object loop over `s2m_net(inputs)`, §8f-3)
   * interact/interaction.py          ScribbleInteraction.predict (GUI: controller + aggregate_wbg(hard))
+
+Five tests execute those reference files and therefore need the reference checkout; they skip where it is absent
+(every clean checkout of this repository, the GPU machines), because the reference's sources may not be copied in:
+  test_reference_fusion_generator_runs_on_our_surface, test_reference_s2m_controller_runs_on_our_network,
+  test_reference_scribble_interaction_runs_on_our_surface, test_pythonpath_overlay_resolves_modules_as_documented,
+  test_reference_davis_processor_runs_on_our_surface.
+test_iou_helpers_equal_the_reference compares against stored outputs of the reference's helpers and runs everywhere.
 """
 import importlib.util
 import os
@@ -20,7 +27,8 @@ import torch
 import abi_emulator
 from oracle import refshim
 
-pytestmark = pytest.mark.skipif(not refshim.available(), reason="/root/reference is only present in the build container")
+# these tests execute the reference's own caller files, which this repository does not contain
+needs_reference = pytest.mark.skipif(not refshim.available(), reason="the reference checkout (MIVOS_REFERENCE_ROOT) is absent")
 REF = refshim.REF_ROOT
 
 
@@ -36,6 +44,7 @@ def rt(monkeypatch):
     return abi_emulator.install_host_runtime(monkeypatch)
 
 
+@needs_reference
 def test_reference_fusion_generator_runs_on_our_surface(rt, prop_sd):
     from oracle import stm_oracle as O, weights as Wt
     from test_gpu_clients import fusion_generator_flow
@@ -60,6 +69,7 @@ def test_reference_fusion_generator_runs_on_our_surface(rt, prop_sd):
     assert float(d.max()) <= 3e-2 and float(d.mean()) <= 1e-3
 
 
+@needs_reference
 def test_reference_s2m_controller_runs_on_our_network(rt, golden):
     from oracle import weights as Wt
     ctl = _load("interact/s2m_controller.py", "_ref_caller_s2m_controller")
@@ -73,6 +83,7 @@ def test_reference_s2m_controller_runs_on_our_network(rt, golden):
     assert m.shape == g["mask"].shape and float((m - torch.from_numpy(g["mask"])).abs().max()) <= 2e-2
 
 
+@needs_reference
 def test_reference_scribble_interaction_runs_on_our_surface(rt, golden, monkeypatch):
     """interact/interaction.py ScribbleInteraction: strokes drawn with cv2 -> controller.interact ->
     aggregate_wbg(hard=True), with our S2MController / S2MNetwork / aggregate behind the reference's imports."""
@@ -101,6 +112,7 @@ def test_reference_scribble_interaction_runs_on_our_surface(rt, golden, monkeypa
     assert float((si.out_prob - prob).abs().max()) <= 2e-2
 
 
+@needs_reference
 def test_pythonpath_overlay_resolves_modules_as_documented():
     """INTEGRATION.md §1: with this repository BEFORE the reference checkout on PYTHONPATH, the modules this
     repository provides resolve here and every other module of the same packages still resolves to the
@@ -125,23 +137,29 @@ def test_pythonpath_overlay_resolves_modules_as_documented():
         assert path.startswith(root if kind == "ours" else REF), ln
 
 
-def test_iou_helpers_equal_the_reference():
-    ref_tu = _load("util/tensor_util.py", "_ref_util_tensor_util")
+def test_iou_helpers_equal_the_reference(golden):
+    """util/tensor_util.py's IoU helpers against the reference's results on the same inputs
+    (oracle/gen_golden_live.py, tests/golden/reference_live*.npz): same values, same element types."""
     from util import tensor_util as ours
+    g = golden("reference_live.npz")
+
+    def same(a, b):
+        a = np.asarray(a.numpy() if torch.is_tensor(a) else a)
+        return a.dtype == b.dtype and np.array_equal(a, b)
+
     rng = np.random.default_rng(3)
     seg_np, gt_np = rng.random((40, 50)) > 0.5, rng.random((40, 50)) > 0.6
     seg_t, gt_t = torch.from_numpy(seg_np), torch.from_numpy(gt_np)
-    for a, b in zip(ours.compute_tensor_iu(seg_t, gt_t), ref_tu.compute_tensor_iu(seg_t, gt_t)):
-        assert a.dtype == b.dtype and float(a) == float(b)
-    assert float(ours.compute_tensor_iou(seg_t, gt_t)) == float(ref_tu.compute_tensor_iou(seg_t, gt_t))
-    assert ours.compute_np_iu(seg_np, gt_np) == ref_tu.compute_np_iu(seg_np, gt_np)
-    assert ours.compute_np_iou(seg_np, gt_np) == ref_tu.compute_np_iou(seg_np, gt_np)
+    assert same(torch.stack(ours.compute_tensor_iu(seg_t, gt_t)), g["iou_tensor_iu"])
+    assert same(ours.compute_tensor_iou(seg_t, gt_t), g["iou_tensor_iou"])
+    assert same(np.stack(ours.compute_np_iu(seg_np, gt_np)), g["iou_np_iu"])
+    assert same(ours.compute_np_iou(seg_np, gt_np), g["iou_np_iou"])
     scores = torch.from_numpy(rng.random((4, 40, 50)).astype(np.float32))
     gt_soft = torch.from_numpy(rng.random((3, 1, 40, 50)).astype(np.float32))
-    assert float(ours.compute_multi_class_iou(scores, gt_soft)) == float(ref_tu.compute_multi_class_iou(scores, gt_soft))
+    assert same(ours.compute_multi_class_iou(scores, gt_soft), g["iou_multi_class"])
     lab, lab2 = rng.integers(0, 4, (40, 50)), rng.integers(0, 4, (40, 50))
-    assert ours.compute_multi_class_iou_idx(lab, gt_soft[:, 0].numpy()) == ref_tu.compute_multi_class_iou_idx(lab, gt_soft[:, 0].numpy())
-    assert ours.compute_multi_class_iou_both_idx(lab, lab2) == ref_tu.compute_multi_class_iou_both_idx(lab, lab2)
+    assert same(ours.compute_multi_class_iou_idx(lab, gt_soft[:, 0].numpy()), g["iou_multi_class_idx"])
+    assert same(ours.compute_multi_class_iou_both_idx(lab, lab2), g["iou_multi_class_both_idx"])
     empty = np.zeros((4, 4), dtype=bool)
     assert ours.compute_np_iou(empty, empty) == 1.0  # 0/0 -> (0 + eps) / (0 + eps)
 
@@ -163,6 +181,7 @@ def _fake_davisinteractive(monkeypatch):
         monkeypatch.setitem(sys.modules, name, mod)
 
 
+@needs_reference
 def test_reference_davis_processor_runs_on_our_surface(rt, ref_outputs, prop_sd, fuse_sd, monkeypatch):
     """davis_processor.py UNCHANGED (the junction between the DAVIS interactive track and InferenceCore:
     S2M per object -> aggregate_wbg(hard) -> update_mask_only x2 -> interact), once on the reference's own

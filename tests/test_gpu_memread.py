@@ -1,5 +1,5 @@
 """GPU: the fused space-time memory read (affinity -> top-k -> softmax -> value read-out) through
-the C ABI, both candidate generators (exact CUDA-core and tcgen05), against
+the C ABI, both candidate generators (exact CUDA-core and tensor-core), against
   * the committed golden vectors produced by the reference's EvalMemoryReader,
   * the float64 oracle (index sets must be IDENTICAL wherever the oracle's k-th/(k+1)-th score gap
     exceeds TIE_EPS = 1e-5; closer than that fp32 summation order decides, also inside the
@@ -129,7 +129,7 @@ def test_cfg2_full_size_properties(dev):
     ("cfg5", 5, 100, 3600, 50),   # BASELINE configs[4]: 720p, 5 objects, 100-frame bank (4.6 GB of bank)
 ])
 def test_full_size_configs_properties(dev, name, K, T, hw, k):
-    """Full-size memory banks of the larger BASELINE configurations: the tcgen05 candidate path and
+    """Full-size memory banks of the larger BASELINE configurations: the tensor-core candidate path and
     the exact SIMT path must select the same slots and produce the same read-out bit for bit;
     size-independent properties: sorted scores, unique indices, convex weights."""
     g = torch.Generator(device=dev).manual_seed(K * 100 + T)

@@ -4,7 +4,7 @@ fixtures generated from the UNMODIFIED reference and against the CPU oracle.
 Stated fp32 tolerance (north_star): the convolution stacks run on the tensor cores in TF32
 (10-bit-mantissa operands, fp32 accumulate, activations stored rounded-to-nearest TF32) while the
 reference computes fp32, so
-  * feature maps        : |d| <= 4e-3 * max|ref|          (measured 1.2e-3 on B200)
+  * feature maps        : |d| <= 4e-3 * max|ref|          (bound of the fp16 / TF32 operand rounding)
   * probabilities       : max |dp| <= 3e-2, mean |dp| <= 1e-3   (measured 1.2e-2 / 1.4e-4)
   * u8 masks            : <= 1 % of pixels differ at low res with random weights, <= 0.1 % at
                           480p (measured 1e-5); fused frames sit on the decision boundary by

@@ -1,16 +1,16 @@
 """Markdown table of the full-size parity runs: reads the drift curves tests/test_gpu_zzz_fullsize.py writes
-(gpurun_out/r02_drift_*.json) and prints one row per case.  Usage: python tools/drift_table.py [dir] > table.md"""
+($MIVOS_DRIFT_DIR/drift_*.json) and prints one row per case.  Usage: python tools/drift_table.py DIR > table.md"""
 import glob
 import json
 import os
 import sys
 
-d = sys.argv[1] if len(sys.argv) > 1 else os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+d = sys.argv[1]
 print("| case | max dp | mean dp | last-frame max dp | mask mismatch worst frame | last frame | decided pixels (mismatching) | max dp per quarter of the clip |")
 print("|---|---|---|---|---|---|---|---|")
-for p in sorted(glob.glob(os.path.join(d, "r02_drift_*.json"))):
+for p in sorted(glob.glob(os.path.join(d, "drift_*.json"))):
     r = json.load(open(p))
-    name = os.path.basename(p)[len("r02_drift_"):-len(".json")]
+    name = os.path.basename(p)[len("drift_"):-len(".json")]
     per = r["dp_max_per_frame"]
     q = max(1, len(per) // 4)
     quarters = " ".join(f"{max(per[i * q:(i + 1) * q if i < 3 else len(per)]):.1e}" for i in range(4))

@@ -1,4 +1,4 @@
-"""Summaries for profiles/: (1) `ncu_summary.py rep <file.ncu-rep>...` prints the key metrics of every
+"""Summaries of Nsight Compute captures: (1) `ncu_summary.py rep <file.ncu-rep>...` prints the key metrics of every
 captured launch from `ncu -i <rep> --page raw --csv`; (2) `ncu_summary.py launches <launches.csv>`
 aggregates a `--metrics gpu__time_duration.sum` launch list by kernel (count, total, share)."""
 import csv, io, subprocess, sys, collections, re
