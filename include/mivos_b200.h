@@ -126,9 +126,14 @@ MIVOS_API int mivos_conv_gemm(const mivos_conv_args* a, mivos_stream_t stream);
  * with `sms` SMs (0: the current device).  Pure host arithmetic: no pointer in `a` is dereferenced
  * (only tested for NULL), no device is needed when sms > 0.                                        */
 MIVOS_API int mivos_conv_plan(const mivos_conv_args* a, int sms, int* bn, int* splits);
-/* Tuning hook: force the output-channel tile width (32/64/128/256; 0 = automatic choice) of the
- * following mivos_conv_gemm calls.  Results do not depend on the tile width (tests/test_gpu_ops.py). */
-MIVOS_API int mivos_conv_tile_override(int bn);
+/* Tuning hook: force the plan of the following mivos_conv_gemm calls (process-wide; mivos_conv_plan
+ * reports it).  (0, 0): automatic choice.  bn = 32/64/128/256, splits = 0: that output-channel tile
+ * width, no split-K.  splits >= 2 (only with bn > 0): also that split-K factor; a call it applies to
+ * then fails unless it attaches a workspace of at least 64 KB + tiles * splits * 128 * bn * 4 bytes
+ * and splits <= taps * cin_pad / k-block (every split owns a non-empty K range).
+ * Results do not depend on the tile width, bit for bit (tests/test_gpu_conv_plans.py); another split-K
+ * factor is another fp32 summation order.                                                             */
+MIVOS_API int mivos_conv_tile_override(int bn, int splits);
 
 /* Gather kernels that feed mivos_conv_gemm ---------------------------------------------------
  * Every HALO-map operator below takes an element-type flag (`f16`, `out_f16`, `src_f16` ...):

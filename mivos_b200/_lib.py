@@ -68,7 +68,7 @@ SIGNATURES = {
     "mivos_store_words": (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _p]),
     "mivos_copy_segments": (_i, [_p, _p, _p, _i, _i, _l, _p]),
     "mivos_conv_gemm": (_i, [C.POINTER(ConvArgs), _p]),
-    "mivos_conv_tile_override": (_i, [_i]),
+    "mivos_conv_tile_override": (_i, [_i, _i]),
     "mivos_conv_plan": (_i, [C.POINTER(ConvArgs), _i, C.POINTER(_i), C.POINTER(_i)]),
     "mivos_stem_gather": (_i, [_p, _p, _i, _i, _i, _p, _i, _i, _i, _l, _l, _p]),
     "mivos_stem_gather_s2d": (_i, [_p, _p, _i, _i, _i, _p, _i, _i, _i, _l, _l, _p]),

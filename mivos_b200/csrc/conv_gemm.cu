@@ -304,6 +304,7 @@ int launch(const mivos_conv_args* a, const ConvParams& p, cudaStream_t stream) {
 using namespace mivos;
 
 namespace mivos {
+// mivos_conv_tile_override: forced tile width (low 16 bits, 0 = automatic) and split-K factor (high bits, 0 or 1 = one pass)
 std::atomic<int> g_tile_override{0};
 }
 
@@ -362,11 +363,23 @@ int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits
     }
   }
   const int forced = g_tile_override.load(std::memory_order_relaxed);
-  if (forced > 0) {
-    MIVOS_REQUIRE((forced == 32 || forced == 64 || forced == 128 || forced == 256) && a->cout_pad % forced == 0,
-                  "conv_gemm: tile override %d does not divide cout_pad %d", forced, a->cout_pad);
-    bn = forced;
+  const int forced_bn = forced & 0xffff, forced_splits = forced >> 16;
+  if (forced_bn > 0) {
+    MIVOS_REQUIRE(a->cout_pad % forced_bn == 0, "conv_gemm: tile override %d does not divide cout_pad %d", forced_bn,
+                  a->cout_pad);
+    bn = forced_bn;
     splits = 1;
+    if (forced_splits >= 2) {
+      // every split must own a non-empty K range, and the partial tiles must fit the caller's workspace
+      const int64_t tiles = mtiles * (a->cout_pad / bn);
+      MIVOS_REQUIRE(forced_splits <= iters_total, "conv_gemm: split-K override %d exceeds the %d k-blocks of the layer",
+                    forced_splits, iters_total);
+      MIVOS_REQUIRE(a->splitk_ws, "conv_gemm: split-K override %d needs a split-K workspace", forced_splits);
+      const int64_t need = kSkCounterBytes + tiles * forced_splits * BM * bn * 4;
+      MIVOS_REQUIRE(need <= a->splitk_ws_bytes, "conv_gemm: split-K override %d x BN %d needs %lld workspace bytes, got %lld",
+                    forced_splits, bn, static_cast<long long>(need), static_cast<long long>(a->splitk_ws_bytes));
+      splits = forced_splits;
+    }
   }
   *bn_out = bn;
   *splits_out = splits;
@@ -384,8 +397,12 @@ extern "C" MIVOS_API int mivos_conv_plan(const mivos_conv_args* a, int sms, int*
   return plan_tiles(a, sms > 0 ? sms : num_sms(), bn, splits);
 }
 
-extern "C" MIVOS_API int mivos_conv_tile_override(int bn) {
-  mivos::g_tile_override.store(bn, std::memory_order_relaxed);
+extern "C" MIVOS_API int mivos_conv_tile_override(int bn, int splits) {
+  MIVOS_REQUIRE(bn == 0 || bn == 32 || bn == 64 || bn == 128 || bn == 256,
+                "conv_tile_override: tile width %d is not 0, 32, 64, 128 or 256", bn);
+  MIVOS_REQUIRE(splits >= 0 && splits <= 0x7fff, "conv_tile_override: bad split-K factor %d", splits);
+  MIVOS_REQUIRE(splits < 2 || bn > 0, "conv_tile_override: a split-K factor (%d) needs a forced tile width", splits);
+  mivos::g_tile_override.store(bn | (splits << 16), std::memory_order_relaxed);
   return MIVOS_OK;
 }
 

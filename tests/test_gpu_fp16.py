@@ -4,6 +4,8 @@ interactive_gui.py:990).  Convolutions are compared against an fp64 convolution 
 fp16-rounded operands: the kernel must be exact up to fp32 accumulation order (2e-5 of the output
 range) plus, for fp16 outputs, one round-to-nearest-even of the result (2^-11 relative).  Copies,
 max pooling and type conversions are bit-exact."""
+import ctypes
+
 import pytest
 import torch
 import torch.nn.functional as F
@@ -16,10 +18,10 @@ H16 = torch.float16
 
 
 def _border_kept(out):
-    """HALO invariant: the one-pixel border of a map stays ZERO.  The register epilogue never touches border rows
-    (the 7 sentinel survives); the TMA epilogue stores whole 32-row boxes and writes the border rows as zeros."""
+    """HALO invariant: no kernel writes the one-pixel border of a map (the 7 sentinel survives), so a border the owner
+    zeroed stays zero.  Both the epilogue and the split-K second pass store interior rows only."""
     for b in (out[:, 0], out[:, -1], out[:, :, 0], out[:, :, -1]):
-        if not bool(((b == 7) | (b == 0)).all()):
+        if not bool((b == 7).all()):
             return False
     return True
 
@@ -173,19 +175,28 @@ def test_memory_read_fp16_output(dev):
     _lib.poll_kernel_error()
 
 
+# (n, h, w, cin, cout, ks) the cost model splits when a workspace is attached, per operand type (every other shape
+# below must keep the single pass); forced split factors of any shape: tests/test_gpu_conv_plans.py
+_SPLITS = {
+    torch.float16: {(1, 30, 54, 1024, 512, 3), (1, 30, 54, 1024, 640, 3), (1, 60, 108, 512, 512, 3)},
+    torch.float32: {(1, 30, 54, 1024, 512, 3), (1, 30, 54, 256, 256, 3), (1, 30, 54, 1024, 640, 3), (1, 60, 108, 512, 512, 3)},
+}
+
+
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])
 @pytest.mark.parametrize("n,h,w,cin,cout,ks,relu,res", [
-    (1, 30, 54, 1024, 512, 3, False, False),   # decoder.compress conv1 / downsample: 14 row tiles, K = 9216
-    (1, 30, 54, 256, 256, 3, True, False),     # layer3 3x3
-    (1, 30, 54, 1024, 256, 1, True, False),    # layer3 1x1 reduce
-    (2, 30, 54, 256, 1024, 1, True, True),     # layer3 1x1 expand + residual, 2 objects
-    (1, 30, 54, 1024, 640, 3, False, False),   # key|value projection (cout_pad 640)
-    (1, 60, 108, 512, 512, 3, False, False),   # 54 row tiles
+    (1, 30, 54, 1024, 512, 3, False, False),   # decoder.compress conv1 / downsample: 14 row tiles, K = 9216; splits
+    (1, 30, 54, 256, 256, 3, True, False),     # layer3 3x3: splits in TF32 only (fp16 keeps BN = 32, S = 1)
+    (1, 30, 54, 1024, 256, 1, True, False),    # layer3 1x1 reduce: S = 1 (enough row tiles)
+    (2, 30, 54, 256, 1024, 1, True, True),     # layer3 1x1 expand + residual, 2 objects: S = 1
+    (1, 30, 54, 1024, 640, 3, False, False),   # key|value projection (cout_pad 640): splits
+    (1, 60, 108, 512, 512, 3, False, False),   # 54 row tiles: splits
 ])
 def test_conv_split_k(dev, dtype, n, h, w, cin, cout, ks, relu, res):
-    """Split-K path of mivos_conv_gemm (taken when a workspace is attached and the cost model prefers
-    it): must agree with the single-pass kernel up to fp32 summation order, with an fp64 convolution
-    of the same rounded operands, and be repeatable on a reused workspace (fixed summation order)."""
+    """Split-K path of mivos_conv_gemm as the cost model plans it on this device when a workspace is attached: the
+    plan must split the shapes of _SPLITS and keep the single pass (bit-identical to the run without workspace) on the
+    others.  Split runs must agree with the single-pass kernel up to fp32 summation order, with an fp64 convolution of
+    the same rounded operands, and be repeatable on a reused workspace (fixed summation order)."""
     g = torch.Generator(device="cpu").manual_seed(cin + cout + ks)
     x = torch.randn((n, cin, h, w), generator=g).to(dev)
     wt = (torch.randn((cout, cin, ks, ks), generator=g) / (cin * ks * ks) ** 0.5).to(dev)
@@ -195,6 +206,16 @@ def test_conv_split_k(dev, dtype, n, h, w, cin, cout, ks, relu, res):
     r = torch.randn((n, cout, h, w), generator=g).to(dev) if res else None
     rh = to_halo(r, pc.cout_pad, dtype) if res else None
     ws = ops.split_k_workspace(dev)
+    a = _lib.ConvArgs()
+    a.n, a.h, a.w, a.taps, a.cin_pad = n, h, w, pc.taps, pc.cin_pad
+    a.cout, a.cout_pad = pc.cout, pc.cout_pad
+    a.in_f16 = a.out_f16 = int(dtype == torch.float16)
+    a.residual = rh.data_ptr() if res else None
+    a.splitk_ws, a.splitk_ws_bytes = ws.data_ptr(), ws.numel()
+    bn, splits = ctypes.c_int(0), ctypes.c_int(0)
+    _lib.check(_lib.load().mivos_conv_plan(ctypes.byref(a), 0, ctypes.byref(bn), ctypes.byref(splits)), "mivos_conv_plan")
+    meant_to_split = (n, h, w, cin, cout, ks) in _SPLITS[dtype]
+    assert (splits.value >= 2) == meant_to_split, f"planned BN={bn.value} S={splits.value}"
     outs = []
     for use_ws in (None, ws, ws, ws):
         out = torch.full((n, h + 2, w + 2, pc.cout_pad), 7.0, device=dev, dtype=dtype)
@@ -203,6 +224,8 @@ def test_conv_split_k(dev, dtype, n, h, w, cin, cout, ks, relu, res):
     torch.cuda.synchronize()
     _lib.poll_kernel_error()
     assert torch.equal(outs[1], outs[2]) and torch.equal(outs[2], outs[3])  # deterministic reduction order
+    if not meant_to_split:
+        assert torch.equal(outs[0], outs[1])  # the same single-pass launch with or without a workspace
     if dtype == torch.float16:
         xr, wr = x.half(), wt.half()
     else:  # kind::tf32 truncates the activations; the packed weights are rounded (rna)

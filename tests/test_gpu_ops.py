@@ -28,15 +28,15 @@ def trunc_tf32(x):
 
 
 @pytest.mark.parametrize("n,h,w,cin,cout,ks,relu,res,dual", [
-    (1, 30, 54, 64, 64, 3, False, False, False),     # BN=64 tile
+    (1, 30, 54, 64, 64, 3, False, False, False),     # 28 row tiles of BN=32 (the plan at 132 SMs)
     (1, 30, 54, 32, 1, 3, False, False, False),      # decoder.pred shape: one real output channel
     (1, 30, 54, 256, 64, 1, True, False, False),     # bottleneck 1x1 + relu
     (2, 60, 108, 128, 128, 3, True, True, False),    # batch 2, residual + relu
-    (1, 120, 216, 256, 256, 3, False, False, True),  # BN=256 tile, dual (raw + relu) output
+    (1, 120, 216, 256, 256, 3, False, False, True),  # 208 tiles of BN=256, dual (raw + relu) output
     (1, 30, 54, 1024, 640, 3, False, False, False),  # fused key|value projection
     (1, 7, 5, 32, 32, 3, False, False, False),       # tiny ragged map (single partial M tile)
-    (1, 120, 216, 64, 128, 1, True, True, True),     # 208 tiles of BN=128 -> persistent kernel, residual+dual
-    (1, 120, 216, 64, 64, 3, True, False, False),    # 208 tiles of BN=64  -> persistent kernel
+    (1, 120, 216, 64, 128, 1, True, True, True),     # 208 tiles of BN=128, residual + dual
+    (1, 120, 216, 64, 64, 3, True, False, False),    # 208 tiles of BN=64 (every tile width: test_gpu_conv_plans.py)
     (1, 240, 432, 32, 20, 3, False, False, False),   # 821 tiles of BN=32, ragged channel tail (20 of 32)
 ])
 def test_conv_gemm(dev, n, h, w, cin, cout, ks, relu, res, dual):

@@ -1,8 +1,8 @@
 """GPU: lock-step propagation of several clips as one batch (mivos_b200/lockstep.py) against the same
 clips propagated one at a time.  The memory read is exact either way; the convolutions of a batch of
-C*K maps may pick another tile width / split-K factor than those of K maps, i.e. another fp32
-accumulation order, so probabilities agree to the conv tolerance of DESIGN.md §6 rather than bit for
-bit; bank bookkeeping is identical; the captured lock-step graph replays the eager launches bit for
+C*K maps may pick another split-K factor than those of K maps, i.e. another fp32 summation order (another
+tile width alone gives the same bits: tests/test_gpu_conv_plans.py), so probabilities agree to the conv
+tolerance of DESIGN.md §6 rather than bit for bit; bank bookkeeping is identical; the captured lock-step graph replays the eager launches bit for
 bit."""
 import numpy as np
 import pytest

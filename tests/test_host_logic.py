@@ -140,6 +140,63 @@ def test_conv_tile_plan_matches_the_on_device_sweep():
     assert plan(8, 30, 54, 1024, 256, 1, ws=True)[1] == 1
 
 
+def test_conv_tile_override_forces_the_plan_and_rejects_invalid_ones():
+    """mivos_conv_tile_override(bn, splits) forces the plan mivos_conv_plan reports (and mivos_conv_gemm runs); a
+    split-K factor the layer cannot take fails loudly instead of falling back, and (0, 0) restores the cost model."""
+    import ctypes as C
+    from mivos_b200 import _lib
+    lib = _lib.load()
+
+    def args(n=1, h=30, w=54, cin=1024, cout=512, taps=9, ws_bytes=48 << 20):
+        a = _lib.ConvArgs()
+        a.n, a.h, a.w, a.taps = n, h, w, taps
+        a.cin_pad, a.cout, a.cout_pad = cin, cout, (cout + 31) // 32 * 32
+        a.in_f16 = a.out_f16 = 1
+        if ws_bytes:
+            a.splitk_ws, a.splitk_ws_bytes = 256, ws_bytes   # never dereferenced by the planner
+        return a
+
+    def plan(a):
+        bn, sp = C.c_int(0), C.c_int(0)
+        rc = lib.mivos_conv_plan(C.byref(a), 132, C.byref(bn), C.byref(sp))
+        return rc, (bn.value, sp.value)
+
+    shapes = [{}, {"cout": 100, "taps": 1, "cin": 64}, {"n": 4, "h": 120, "w": 216, "cin": 64, "cout": 64}]
+    auto = [plan(args(**sh)) for sh in shapes]
+    assert all(rc == 0 for rc, _ in auto) and auto[0][1][1] >= 2  # decoder.compress splits on its own
+    # decoder.compress (1, 30, 54, 1024 -> 512, 3x3, fp16): 32 x 56 HALO rows = 14 row tiles, 9 taps x 16 = 144 k-blocks
+    m_tiles, kblocks = 14, 144
+    try:
+        for bn in (32, 64, 128, 256):
+            assert lib.mivos_conv_tile_override(bn, 0) == 0
+            assert plan(args()) == (0, (bn, 1))
+            for sp in (2, 3, 5, 7, 8, kblocks):
+                assert lib.mivos_conv_tile_override(bn, sp) == 0
+                assert plan(args(ws_bytes=1 << 40)) == (0, (bn, sp)), (bn, sp)
+        assert lib.mivos_conv_tile_override(128, 1) == 0 and plan(args()) == (0, (128, 1))
+        # rejected by the hook itself; the previous override stays in force
+        assert lib.mivos_conv_tile_override(64, 3) == 0
+        for bad in ((0, 2), (48, 0), (512, 0), (-32, 0), (64, -1)):
+            assert lib.mivos_conv_tile_override(*bad) == -1, bad
+            assert b"conv_tile_override" in lib.mivos_last_error()
+            assert plan(args()) == (0, (64, 3))
+        # rejected for the layer by the planner (so mivos_conv_gemm fails the same way)
+        assert lib.mivos_conv_tile_override(64, kblocks + 1) == 0               # a split with an empty K range
+        assert plan(args(ws_bytes=1 << 40))[0] == -1 and b"k-blocks" in lib.mivos_last_error()
+        assert lib.mivos_conv_tile_override(128, 2) == 0                        # 1x1 over 64 channels: one k-block
+        assert plan(args(cout=100, taps=1, cin=64))[0] == -1 and b"k-blocks" in lib.mivos_last_error()
+        assert lib.mivos_conv_tile_override(64, 2) == 0
+        assert plan(args(ws_bytes=0))[0] == -1 and b"workspace" in lib.mivos_last_error()
+        need = 65536 + m_tiles * (512 // 64) * 2 * 128 * 64 * 4
+        assert plan(args(ws_bytes=need)) == (0, (64, 2))
+        assert plan(args(ws_bytes=need - 1))[0] == -1 and b"workspace" in lib.mivos_last_error()
+        assert lib.mivos_conv_tile_override(256, 0) == 0                        # 256 does not divide cout_pad 128
+        assert plan(args(cout=100, taps=1, cin=64))[0] == -1 and b"cout_pad" in lib.mivos_last_error()
+    finally:
+        assert lib.mivos_conv_tile_override(0, 0) == 0
+    assert [plan(args(**sh)) for sh in shapes] == auto
+
+
 def test_attention_read_network_checkpoint_surface(prop_sd):
     """model/attn_network.py:30-41 + fusion_model.py:187: same sub-module names as the propagation
     network minus the decoder, so a propagation checkpoint loads with strict=False and nothing is

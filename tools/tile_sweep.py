@@ -44,7 +44,7 @@ for (n, h, w, cin, cout, ks, res) in SHAPES:
         if bn and pc.cout_pad % bn:
             row.append("   -  ")
             continue
-        lib.mivos_conv_tile_override(bn)
+        lib.mivos_conv_tile_override(bn, 0)
         ops.conv_gemm(x, pc, n, h, w, out, relu=True, residual=r)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
@@ -60,7 +60,7 @@ for (n, h, w, cin, cout, ks, res) in SHAPES:
         e1.record()
         torch.cuda.synchronize()
         row.append(f"{1e3 * e0.elapsed_time(e1) / (3 * REPS):6.1f}")
-    lib.mivos_conv_tile_override(0)
+    lib.mivos_conv_tile_override(0, 0)
     fl = 2.0 * n * h * w * ks * ks * cin * cout
     best = min(float(v) for v in row[1:] if v.strip() != "-")
     print(f"n={n} {h:3d}x{w:3d} {cin:4d}->{cout:4d} k{ks} res={int(res)} | auto {row[0]} | 32:{row[1]} 64:{row[2]} 128:{row[3]} 256:{row[4]} | best {fl / best / 1e6:7.1f} TF/s")
