@@ -9,6 +9,7 @@
 #include "pdl.cuh"
 
 #include <atomic>
+#include <mutex>
 
 namespace mivos {
 extern std::atomic<int64_t> g_launches;
@@ -142,6 +143,24 @@ __global__ void upsample16_kernel(const float* __restrict__ maps, int h16, int w
   }
 }
 
+// Dynamic shared memory of attention_kernel: the query tile plus one logit row per query.
+constexpr int kMaxAttentionSmem = 220 * 1024;  // hw <= 6912
+inline int64_t attention_smem(int64_t hw) { return (QB * 128 + QB * hw) * 4; }
+
+// Both entry points launch attention_kernel, so they share one record of its opt-in limit.  The
+// attribute is only ever raised: lowering it for a smaller request would make a later launch of a
+// size in between fail, since that size had already been allowed.
+std::mutex g_attention_smem_mu;
+int g_attention_smem = 0;
+
+cudaError_t reserve_attention_smem(int smem) {
+  std::lock_guard<std::mutex> lock(g_attention_smem_mu);
+  if (smem <= g_attention_smem) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e == cudaSuccess) g_attention_smem = smem;
+  return e;
+}
+
 }  // namespace
 }  // namespace mivos
 
@@ -154,20 +173,18 @@ extern "C" MIVOS_API int mivos_attention_map(const float* mk, const float* qk, i
   MIVOS_REQUIRE(mk && qk && pos && neg && out && scratch, "attention_map: null pointer");
   MIVOS_REQUIRE((reinterpret_cast<uintptr_t>(mk) & 15) == 0 && (reinterpret_cast<uintptr_t>(qk) & 15) == 0,
                 "attention_map: mk/qk must be 16-byte aligned");
+  MIVOS_REQUIRE(h16 > 0 && w16 > 0, "attention_map: bad key grid %d x %d", h16, w16);
+  MIVOS_REQUIRE(attention_smem(static_cast<int64_t>(h16) * w16) <= kMaxAttentionSmem,
+                "attention_map: %d x %d key pixels exceed the shared-memory tile", h16, w16);
   const int hw = h16 * w16;
-  const int smem = (QB * 128 + QB * hw) * 4;
-  MIVOS_REQUIRE(hw > 0 && smem <= 220 * 1024, "attention_map: %d key pixels exceed the shared-memory tile", hw);
+  const int smem = static_cast<int>(attention_smem(hw));
   // scratch: pooled[2][hw] followed by maps[2][hw]
   float* pooled = scratch;
   float* maps = scratch + 2 * hw;
   launch_pdl(area_pool16_kernel, ceil_div(2 * hw, 128), 128, 0, stream, pos, neg, h16, w16, pooled);
   g_launches.fetch_add(1);
   MIVOS_CUDA_OK(cudaGetLastError());
-  static int configured_smem = 0;
-  if (smem > configured_smem) {
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured_smem = smem;
-  }
+  MIVOS_CUDA_OK(reserve_attention_smem(smem));
   launch_pdl(attention_kernel, ceil_div(hw, QB), ATT_THREADS, smem, stream, mk, qk, hw, pooled, maps,
              static_cast<float*>(nullptr));
   g_launches.fetch_add(1);
@@ -190,14 +207,11 @@ extern "C" MIVOS_API int mivos_attention_weights(const float* mk, const float* q
   MIVOS_REQUIRE(mk && qk && w_out && scratch, "attention_weights: null pointer");
   MIVOS_REQUIRE((reinterpret_cast<uintptr_t>(mk) & 15) == 0 && (reinterpret_cast<uintptr_t>(qk) & 15) == 0,
                 "attention_weights: mk/qk must be 16-byte aligned");
-  const int smem = (QB * 128 + QB * hw) * 4;
-  MIVOS_REQUIRE(hw > 0 && smem <= 220 * 1024, "attention_weights: %d key pixels exceed the shared-memory tile", hw);
+  MIVOS_REQUIRE(hw > 0 && attention_smem(hw) <= kMaxAttentionSmem,
+                "attention_weights: %d key pixels exceed the shared-memory tile", hw);
+  const int smem = static_cast<int>(attention_smem(hw));
   MIVOS_CUDA_OK(cudaMemsetAsync(scratch, 0, static_cast<size_t>(2) * hw * 4, stream));  // pooled = 0: maps unused
-  static int configured_smem = 0;
-  if (smem > configured_smem) {
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured_smem = smem;
-  }
+  MIVOS_CUDA_OK(reserve_attention_smem(smem));
   launch_pdl(attention_kernel, ceil_div(hw, QB), ATT_THREADS, smem, stream, mk, qk, hw, scratch, scratch + 2 * hw, w_out);
   g_launches.fetch_add(1);
   MIVOS_CUDA_OK(cudaGetLastError());

@@ -434,6 +434,9 @@ def attention_map(mk: torch.Tensor, qk: torch.Tensor, h16: int, w16: int, pos: t
                   neg: torch.Tensor) -> torch.Tensor:
     """mk, qk pixel-major [hw,128]; pos/neg [1,1,H,W] -> [1,2,H,W]."""
     _req(mk), _req(qk), _req(pos), _req(neg)
+    for t in (pos, neg):
+        if tuple(t.shape) != (1, 1, 16 * h16, 16 * w16):
+            raise _lib.MivosError(f"attention_map: pos/neg {tuple(t.shape)} are not [1,1,{16 * h16},{16 * w16}]")
     out = torch.empty((1, 2, h16 * 16, w16 * 16), dtype=torch.float32, device=mk.device)
     scratch = torch.empty(4 * h16 * w16, dtype=torch.float32, device=mk.device)
     check(_lib.lib().mivos_attention_map(_ptr(mk), _ptr(qk), h16, w16, _ptr(pos), _ptr(neg), _ptr(out),
@@ -445,6 +448,8 @@ def attention_weights(mk: torch.Tensor, qk: torch.Tensor) -> torch.Tensor:
     """mk, qk pixel-major [hw,128] -> W [hw (memory), hw (query)]: softmax over the memory axis (get_W)."""
     _req(mk), _req(qk)
     hw = mk.shape[0]
+    if mk.dim() != 2 or mk.shape[1] != 128 or qk.shape != mk.shape:
+        raise _lib.MivosError(f"attention_weights: mk {tuple(mk.shape)} / qk {tuple(qk.shape)} are not both [hw,128]")
     out = torch.empty((hw, hw), dtype=torch.float32, device=mk.device)
     scratch = torch.empty(4 * hw, dtype=torch.float32, device=mk.device)
     check(_lib.lib().mivos_attention_weights(_ptr(mk), _ptr(qk), hw, _ptr(out), _ptr(scratch), _stream()),

@@ -67,6 +67,12 @@ def test_argument_validation_fails_loudly_without_touching_a_device():
     assert lib.mivos_overlay_davis(one, one, 1, 4, 4, one, 7, C.c_double(1.5), 0, one, null) == -1
     assert b"alpha" in lib.mivos_last_error()
     assert lib.mivos_overlay_davis(one, one, 1, 4, 4, one, 0, C.c_double(0.5), 0, one, null) == -1
+    assert lib.mivos_attention_map(one, one, -1, -1, one, one, one, one, null) == -1  # negative grid, positive product
+    assert b"attention_map" in lib.mivos_last_error()
+    assert lib.mivos_attention_map(one, one, 64, 109, one, one, one, one, null) == -1  # 6976 keys: above the 220 KB tile
+    assert b"attention_map" in lib.mivos_last_error()
+    assert lib.mivos_attention_weights(one, one, 6976, one, one, null) == -1
+    assert b"attention_weights" in lib.mivos_last_error()
     a = _lib.ConvArgs()
     assert lib.mivos_conv_gemm(C.byref(a), null) == -1 and b"conv_gemm" in lib.mivos_last_error()
     with __import__("pytest").raises(_lib.MivosError):
