@@ -61,6 +61,19 @@ def test_argument_validation_fails_loudly_without_touching_a_device():
     assert lib.mivos_gather_dilated(one, 1, 4, 4, 30, 32, 2, one, 288, 1, null) == -1  # c not a multiple of the vector width
     assert lib.mivos_stem_gather_frames(one, 1, 4, 32, 32, one, 320, 1, null) == -1  # 4 input channels
     assert b"3 or 6" in lib.mivos_last_error()
+    # the first frame width each stem gather refuses for want of shared memory (227 KB per CTA); the width 2 below is
+    # the widest admitted, tests/test_gpu_ops_ragged.py runs it for the 6-channel fp32 form
+    for w, cin, f16 in ((2762, 3, 0), (5530, 3, 1), (1656, 5, 0), (3316, 5, 1)):
+        masks = one if cin == 5 else null
+        assert lib.mivos_stem_gather(one, masks, 1, 2, w, one, 256, f16, 1, 0, 0, null) == -1, (w, cin, f16)
+        assert b"shared memory" in lib.mivos_last_error()
+    for w, cin, f16 in ((9678, 3, 0), (19364, 3, 1), (5804, 5, 0), (11616, 5, 1)):
+        masks = one if cin == 5 else null
+        assert lib.mivos_stem_gather_s2d(one, masks, 1, 2, w, one, 96, f16, 1, 0, 0, null) == -1, (w, cin, f16)
+        assert b"shared memory" in lib.mivos_last_error()
+    for w, f16 in ((1378, 0), (2762, 1)):
+        assert lib.mivos_stem_gather_frames(one, 1, 6, 2, w, one, 320, f16, null) == -1, (w, f16)
+        assert b"shared memory" in lib.mivos_last_error()
     assert lib.mivos_halo_avgpool_broadcast(one, 1, 4, 4, 64, 64, 8, one, 64, 0, 1, null) == -1  # window beyond the stride
     assert lib.mivos_upsample_bilinear(one, 1, 0, 4, 32, 0, one, 8, 8, 32, 0, 32, 0, null) == -1
     assert lib.mivos_halo_upsample_to_plane(one, 1, 4, 4, 32, 32, 16, 16, 0, one, null) == -1  # coff == cstride

@@ -269,3 +269,46 @@ def test_full_size_configs_properties(dev, name, K, T, hw, k):
         ref = torch.topk(aff, k).indices.sort()[0]
         assert torch.equal(i_tc[o, q].long().sort()[0], ref)
     _lib.poll_kernel_error()
+
+
+@pytest.mark.parametrize("q_div", [0, 3])
+def test_read_into_halo_window(dev, q_div):
+    """The read as the decoder takes it (engine.py): written straight into channels [256, 768) of a 1024-channel HALO
+    concat map, fp32 or fp16, for K = 3 objects and a ragged 7 x 9 query map.  q_div = 0: the K objects read one
+    query set; q_div = K: two clips of K objects, each with its own set, in one call.  The map is pre-filled with a
+    sentinel that must survive on the border and outside the window; the fp16 map holds the fp32 result rounded once."""
+    K, h, w, T, k, coff, sent = 3, 7, 9, 4, 20, 256, 7.0
+    hw, slots = h * w, T * h * w
+    sets = 2 if q_div else 1
+    objs = K * sets
+    g = torch.Generator().manual_seed(40 + q_div)
+    bk = torch.randn((objs, slots, 128), generator=g).to(dev)
+    bv = torch.randn((objs, slots, 512), generator=g).to(dev)
+    qk = torch.randn((sets, hw, 128), generator=g).to(dev)
+    # float64 reference (as in test_generators_agree_bit_for_bit_and_match_f64); object o reads set o // q_div
+    qo = qk[torch.arange(objs, device=dev) // K] if q_div else qk[0].expand(objs, hw, 128)
+    aff = torch.einsum("ksc,kqc->ksq", bk.double(), (qo / (128 ** 0.5)).double())
+    vals, ind = torch.topk(aff, k + 1, dim=1)
+    gap = vals[:, k - 1] - vals[:, k]
+    e = torch.exp(vals[:, :k] - vals[:, :1])
+    ref = torch.einsum("kjq,kjqc->kqc", e / e.sum(1, keepdim=True),
+                       bv.double()[torch.arange(objs, device=dev)[:, None, None], ind[:, :k]])
+    inside = torch.zeros((objs, h + 2, w + 2, 1024), dtype=torch.bool, device=dev)
+    inside[:, 1:-1, 1:-1, coff:coff + 512] = True
+    for algo in ALGOS:
+        got = {}
+        for dt in (torch.float32, torch.float16):
+            out = torch.full((objs, h + 2, w + 2, 1024), sent, dtype=dt, device=dev)
+            _, idx, _ = ops.memory_read(bk, bv, slots, qk if q_div else qk[0], k, out, out_coff=coff, halo_hw=(h, w),
+                                        algo=algo, want_topk=True, q_div=q_div)
+            torch.cuda.synchronize()
+            _lib.poll_kernel_error()
+            assert bool((out[~inside] == sent).all()), (algo, dt, "written outside the window")
+            got[dt] = out[:, 1:-1, 1:-1, coff:coff + 512].reshape(objs, hw, 512)
+        assert torch.equal(got[torch.float16], got[torch.float32].half()), algo
+        same = (idx.long().transpose(1, 2).sort(1)[0] == ind[:, :k].sort(1)[0]).all(1)
+        assert bool(same[gap > TIE_EPS].all()), algo
+        ok = same & (gap > TIE_EPS)
+        err = float((got[torch.float32].double() - ref)[ok].abs().max()) / float(ref.abs().max())
+        print(f"memory read into a HALO window, algo {algo} q_div={q_div}: max err / range = {err:.3g} (bound 2e-5)")
+        assert err <= 2e-5

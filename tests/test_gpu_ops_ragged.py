@@ -1,5 +1,6 @@
-"""GPU: the propagation-path elementwise, layout and attention kernels (csrc/elementwise.cu, csrc/halo_ops.cu,
-csrc/attention.cu) at ragged shapes and edge inputs, against plain float64 statements of the same operations.
+"""GPU: the propagation-path elementwise, layout, attention and stem-gather kernels (csrc/elementwise.cu,
+csrc/halo_ops.cu, csrc/attention.cu) at ragged shapes and edge inputs, against plain float64 statements of the same
+operations; and the graph-staging kernels (store_i32, store_words, copy_segments) bit for bit.
 
 Every reference is computed from the operands the kernel saw (fp16-rounded where the map is fp16; the kernel's
 own fp32 intermediate output where a stage is checked on its own).  Copies, gathers, pooling and argmax are
@@ -517,3 +518,263 @@ def test_halo_sigmoid_to_plane_ragged(dev):
     # (at most 6u relative: within 4 to 6 ulp of the fp32 result)
     _check("halo_sigmoid_to_plane", plane[:-1], ref, ref * (2 * U + 4 * U * (1 - ref)))
     assert float(plane[-1]) == SENT
+
+
+# ------------------------------------------------------------------------------------------------ stem gathers
+def stem_images(frames, masks=None):
+    """fp64 input images of a stem gather [N, cin, H, W] and the bound of each value.  frames alone: a batch of
+    3- or 6-channel images.  frames [G, 3, H, W] with masks [G, K, H, W]: per object (group-major) the frame, its own
+    mask and the exact sum of the other objects' masks.  The kernel adds the K - 1 other masks to 0 in object order,
+    the first addition exact: |others - sum| <= (K - 2) u sum_{j != k} m_j.  Every other channel is one rounding of
+    the fp32 operand to the map type, applied by the caller."""
+    if masks is None:
+        img = frames.double()
+        return img, torch.zeros_like(img)
+    G, K = masks.shape[:2]
+    m = masks.double()
+    imgs, bounds = [], []
+    for k in range(K):
+        others = torch.cat([m[:, :k], m[:, k + 1:]], 1).sum(1, keepdim=True)
+        imgs.append(torch.cat([frames.double(), m[:, k:k + 1], others], 1))
+        b = torch.zeros_like(imgs[-1])
+        b[:, 4:] = max(K - 2, 0) * U * others
+        bounds.append(b)
+    N = G * K
+    return torch.stack(imgs, 1).reshape(N, 5, *frames.shape[2:]), torch.stack(bounds, 1).reshape(N, 5, *frames.shape[2:])
+
+
+def stem_matrix(img, kpad, s2d):
+    """The gather of img [N, cin, H, W] as the kernels write it: HALO rows of the half-resolution output map, kpad
+    columns.  49 taps: the F.unfold(7, stride 2, pad 3) windows in (ky, kx, c) order.  s2d (header formula):
+    out[row(Y, X), py*8*cin + j*cin + c] = in[c, 2Y + py, 2X - 4 + j], zero outside the image.  Border rows and the
+    pad columns are zero."""
+    N, cin, H, W = img.shape
+    ho, wo = H // 2, W // 2
+    if s2d:
+        p = F.pad(img, (4, 4))
+        cols = torch.stack([p[:, :, py::2, j:j + 2 * wo:2] for py in range(2) for j in range(8)], 1)  # [N, 16, cin, ho, wo]
+        cols = cols.permute(0, 3, 4, 1, 2).reshape(N, ho, wo, 16 * cin)
+    else:
+        cols = F.unfold(img, 7, padding=3, stride=2).reshape(N, cin, 49, ho, wo).permute(0, 3, 4, 2, 1)
+        cols = cols.reshape(N, ho, wo, 49 * cin)
+    out = torch.zeros((N, ho + 2, wo + 2, kpad), dtype=torch.float64, device=img.device)
+    out[:, 1:-1, 1:-1, :cols.shape[-1]] = cols
+    return out.reshape(-1, kpad)
+
+
+def _stem_out(N, H, W, kpad, dtype, dev):
+    """A matrix of N * (H/2 + 2) * (W/2 + 2) rows filled with the sentinel, plus one guard row past its end."""
+    rows = N * (H // 2 + 2) * (W // 2 + 2)
+    buf = torch.full((rows + 1, kpad), SENT, dtype=dtype, device=dev)
+    return buf, buf[:rows]
+
+
+def _check_stem(what, buf, img, bound, kpad, s2d, dtype):
+    """Channels other than "others": bit-exact after one rounding to the map type.  "others" (channel 4 of the mask
+    form, K >= 3): within its bound, exact where that is 0 (zero padding).  Guard row untouched."""
+    cin = img.shape[1]
+    assert bool((buf[-1] == SENT).all()), f"{what}: wrote past the matrix"
+    got = buf[:-1].double()
+    rounded = img.to(dtype).double()
+    if bound.any():  # the "others" channel keeps its exact sum, the other channels their rounded value
+        rounded[:, 4] = img[:, 4]
+    ref = stem_matrix(rounded, kpad, s2d)
+    if not bound.any():
+        assert torch.equal(got, ref), what
+        return
+    bnd = _round16(stem_matrix(bound, kpad, s2d), ref, dtype)
+    col = torch.arange(kpad, device=buf.device)
+    oc = (col < (16 if s2d else 49) * cin) & (col % cin == 4)
+    assert torch.equal(got[:, ~oc], ref[:, ~oc]), f"{what}: frame / own-mask / pad columns"
+    go, ro, bo = got[:, oc], ref[:, oc], bnd[:, oc]
+    live = (ro != 0) | (bo != 0)
+    assert torch.equal(go[~live], ro[~live]), f"{what}: others in the zero padding"
+    _check(f"{what} others", go[live], ro[live], bo[live])
+
+
+def _round16(bound, ref, dtype):
+    """A bound on an fp32 value, widened by its final rounding to an fp16 map (2^-25 absolute below the normal range)."""
+    if dtype != H16:
+        return bound
+    return bound * (1 + 2.0 ** -11) + 2.0 ** -11 * ref.abs() + 2.0 ** -25
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, H16])
+@pytest.mark.parametrize("s2d", [False, True])
+@pytest.mark.parametrize("K", [1, 2, 16])
+def test_stem_gather_masks_ragged(dev, dtype, s2d, K):
+    """The memorize stem: frame + K masks -> per object (frame, own mask, others).  One group at h = 2 (a single
+    output row), w = 2 and a ragged 14 x 22; three groups whose frames and masks lie frame_gstride / mask_gstride
+    apart with NaN in the gaps between the clips."""
+    kpad = 96 if s2d else 256  # 16 * 5 = 80 / 49 * 5 = 245 gathered columns: the rest must be written as zeros
+    fn = _lib.lib().mivos_stem_gather_s2d if s2d else _lib.lib().mivos_stem_gather
+    g = torch.Generator().manual_seed(K * 10 + int(s2d))
+    for G, H, W in ((1, 2, 10), (1, 6, 2), (1, 14, 22), (3, 6, 10)):
+        hw = H * W
+        frames = torch.randn(G, 3, H, W, generator=g)
+        masks = torch.rand(G, K, H, W, generator=g)
+        fgs, mgs = (3 * hw + hw + 7, K * hw + hw + 5) if G > 1 else (0, 0)
+        fbuf = torch.full((max(G * fgs, 3 * hw),), NAN)
+        mbuf = torch.full((max(G * mgs, K * hw),), NAN)
+        for gi in range(G):
+            fbuf[gi * fgs:gi * fgs + 3 * hw] = frames[gi].reshape(-1)
+            mbuf[gi * mgs:gi * mgs + K * hw] = masks[gi].reshape(-1)
+        fbuf, mbuf = fbuf.to(dev), mbuf.to(dev)
+        buf, out = _stem_out(G * K, H, W, kpad, dtype, dev)
+        _lib.check(fn(ops._ptr(fbuf), ops._ptr(mbuf), K, H, W, ops._ptr(out), kpad, ops._f16(out), G, fgs, mgs,
+                      ops._stream()), "stem_gather")
+        torch.cuda.synchronize()
+        _lib.poll_kernel_error()
+        img, bound = stem_images(frames.to(dev), masks.to(dev))
+        _check_stem(f"stem_gather s2d={s2d} {dtype} K={K} G={G} {H}x{W}", buf, img, bound, kpad, s2d, dtype)
+        if G == 1:  # the wrapper's [K, 1, H, W] form is the same launch
+            buf2, out2 = _stem_out(K, H, W, kpad, dtype, dev)
+            ops.stem_gather(frames.to(dev), masks[0, :, None].contiguous().to(dev), out2, s2d=s2d)
+            assert torch.equal(buf2, buf)
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, H16])
+def test_stem_gather_frames_ragged(dev, dtype):
+    """Batches of frames: cin 3 through mivos_stem_gather (49 taps and s2d) and mivos_stem_gather_frames, cin 6 (the
+    S2M stem: image, previous mask, +/- scribbles) through mivos_stem_gather_frames; h = 2, w = 2, ragged, and the
+    widest 6-channel frame the shared-memory check admits, 1376 pixels in fp32 (7 rows x 1382 x 6 x 4 B = 232344 B
+    of the 232448) and 2760 in fp16."""
+    g = torch.Generator().manual_seed(6)
+    widest = 1376 if dtype == torch.float32 else 2760
+    for cin in (3, 6):
+        for n, H, W in ((2, 2, 2), (2, 2, 14), (2, 10, 2), (2, 6, 22)) + (((1, 2, widest),) if cin == 6 else ()):
+            frames = torch.randn(n, cin, H, W, generator=g).to(dev)
+            img, bound = stem_images(frames)
+            kpad = 160 if cin == 3 else 320
+            buf, out = _stem_out(n, H, W, kpad, dtype, dev)
+            ops.stem_gather_frames(frames, out)
+            torch.cuda.synchronize()
+            _lib.poll_kernel_error()
+            _check_stem(f"stem_gather_frames cin={cin} {dtype} n={n} {H}x{W}", buf, img, bound, kpad, False, dtype)
+            if cin == 3:
+                for s2d, kp in ((False, kpad), (True, 56)):
+                    buf, out = _stem_out(n, H, W, kp, dtype, dev)
+                    ops.stem_gather(frames, None, out, s2d=s2d)
+                    torch.cuda.synchronize()
+                    _check_stem(f"stem_gather s2d={s2d} cin=3 {dtype} n={n} {H}x{W}", buf, img, bound, kp, s2d, dtype)
+
+
+# ------------------------------------------------------------------------------------------------ graph staging
+# Every replayed frame depends on these (inference_core.py, lockstep.py): the int32 bank counters, the pointer table
+# of the frame, and the copies that stage its operands and deliver its result planes.  All bit-exact, with sentinels
+# on both sides of every destination.
+I32_SENT, I64_SENT, BSENT = -7, -0x0123456789ABCDEF, 0xA5
+GUARD = 256  # sentinel bytes on each side of a copy destination (keeps the payload 16-byte aligned)
+
+
+def test_store_i32_ragged(dev):
+    vals = [2 ** 31 - 1, -2 ** 31, 0, 12345]
+    buf = torch.empty(8, dtype=torch.int32, device=dev)
+    for n in range(1, 5):
+        buf.fill_(I32_SENT)
+        ops.store_i32(buf[2:], *vals[:n])
+        exp = torch.full((8,), I32_SENT, dtype=torch.int32)
+        exp[2:2 + n] = torch.tensor(vals[:n], dtype=torch.int32)
+        assert torch.equal(buf.cpu(), exp), n
+
+
+def test_store_words_ragged(dev):
+    """n64 = 0, 1, 37, 64 words with n32 = 0..4 counters; 130 words take three launches of the wrapper (64 + 64 + 2),
+    the counters going with the first."""
+    import random
+    rnd = random.Random(5)
+    b64 = torch.empty(134, dtype=torch.int64, device=dev)
+    b32 = torch.empty(8, dtype=torch.int32, device=dev)
+    for n64, n32s in ((0, range(5)), (1, range(5)), (37, range(5)), (64, range(5)), (130, (0, 4))):
+        for n32 in n32s:
+            w64 = [rnd.getrandbits(64) - 2 ** 63 for _ in range(n64)]
+            w32 = [rnd.getrandbits(32) - 2 ** 31 for _ in range(n32)]
+            b64.fill_(I64_SENT), b32.fill_(I32_SENT)
+            ops.store_words(b64[2:], w64, b32[2:], w32)
+            e64 = torch.full((134,), I64_SENT, dtype=torch.int64)
+            e64[2:2 + n64] = torch.tensor(w64, dtype=torch.int64)
+            e32 = torch.full((8,), I32_SENT, dtype=torch.int32)
+            e32[2:2 + n32] = torch.tensor(w32, dtype=torch.int32)
+            assert torch.equal(b64.cpu(), e64) and torch.equal(b32.cpu(), e32), (n64, n32)
+
+
+def _guarded(nbytes, dev):
+    """(buffer, payload): nbytes payload bytes between GUARD sentinel bytes on each side, inside one allocation."""
+    buf = torch.full((nbytes + 2 * GUARD,), BSENT, dtype=torch.uint8, device=dev)
+    return buf, buf[GUARD:GUARD + nbytes]
+
+
+def _i64(vals, dev):
+    return torch.tensor(vals, dtype=torch.int64, device=dev)
+
+
+@pytest.mark.parametrize("dyn_is_src", [True, False])
+def test_copy_segments_ragged(dev, dyn_is_src):
+    """Segments of 16 B, 4 KB + 16 B, 20 MB (longer than one grid-stride sweep, about 8.6 MB on 132 SMs) and two
+    other sizes, all different and below max_bytes; a sixth segment has dyn = 0 and must copy nothing, in particular
+    not onto its fixed side."""
+    sizes = [16, 4096 + 16, 20 << 20, 160, 65536 + 48, 4096]
+    skip = len(sizes) - 1
+    gen = torch.Generator(device=dev).manual_seed(7)
+    srcs = [torch.randint(0, 256, (s,), dtype=torch.uint8, device=dev, generator=gen) for s in sizes]
+    dsts = [_guarded(s, dev) for s in sizes]
+    src_p = [s.data_ptr() for s in srcs]
+    dst_p = [p.data_ptr() for _, p in dsts]
+    fixed, dyn = (dst_p, src_p) if dyn_is_src else (src_p, dst_p)
+    dyn = [0 if i == skip else p for i, p in enumerate(dyn)]
+    ops.copy_segments(_i64(fixed, dev), _i64(dyn, dev), _i64(sizes, dev), len(sizes), dyn_is_src, (20 << 20) + 4096)
+    torch.cuda.synchronize()
+    _lib.poll_kernel_error()
+    for i, (buf, payload) in enumerate(dsts):
+        g0, g1 = buf[:GUARD], buf[GUARD + sizes[i]:]
+        assert bool((g0 == BSENT).all() and (g1 == BSENT).all()), f"segment {i} ({sizes[i]} B) overran its destination"
+        if i == skip:
+            assert bool((payload == BSENT).all()), "a skipped segment wrote its destination"
+        else:
+            assert torch.equal(payload, srcs[i]), f"segment {i} ({sizes[i]} B)"
+
+
+def test_copy_segments_graph_replay(dev):
+    """A frame step as inference_core.py records it: ONE captured graph stages three segments into fixed buffers
+    (dyn sources) and delivers them again (dyn destinations); between replays store_words rewrites the pointer table.
+    The third replay skips segment 1 both ways (pointer 0): its staging buffer keeps the previous frame's bytes."""
+    sizes = [16, 4096 + 16, 1 << 20]
+    n = len(sizes)
+    gen = torch.Generator(device=dev).manual_seed(8)
+    stage = [_guarded(s, dev) for s in sizes]
+    fixed = _i64([p.data_ptr() for _, p in stage], dev)
+    nbytes = _i64(sizes, dev)
+    table = torch.zeros(2 * n, dtype=torch.int64, device=dev)  # [sources..., destinations...]
+    frames = [([torch.randint(0, 256, (s,), dtype=torch.uint8, device=dev, generator=gen) for s in sizes],
+               [_guarded(s, dev) for s in sizes]) for _ in range(4)]
+
+    def step(f, skip=None):
+        srcs, dsts = frames[f]
+        ptrs = [0 if i == skip else s.data_ptr() for i, s in enumerate(srcs)]
+        ptrs += [0 if i == skip else p.data_ptr() for i, (_, p) in enumerate(dsts)]
+        ops.store_words(table, ptrs)
+
+    def body():
+        ops.copy_segments(fixed, table[:n], nbytes, n, True, max(sizes))
+        ops.copy_segments(fixed, table[n:], nbytes, n, False, max(sizes))
+
+    def check(f, skip=None, kept=None):
+        torch.cuda.synchronize()
+        _lib.poll_kernel_error()
+        srcs, dsts = frames[f]
+        for i in range(n):
+            want = kept if i == skip else srcs[i]
+            for buf, payload, sent in ((*stage[i], want), (*dsts[i], None if i == skip else srcs[i])):
+                assert bool((buf[:GUARD] == BSENT).all() and (buf[GUARD + sizes[i]:] == BSENT).all()), (f, i)
+                assert bool((payload == BSENT).all()) if sent is None else torch.equal(payload, sent), (f, i)
+
+    step(0)
+    body()  # eagerly once, as InferenceCore does before capturing
+    check(0)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        body()
+    for f, skip in ((1, None), (2, 1), (3, None)):
+        step(f, skip)
+        graph.replay()
+        check(f, skip, kept=frames[f - 1][0][1])

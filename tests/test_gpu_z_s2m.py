@@ -1,17 +1,31 @@
-"""GPU: SURVEY §8(f) row 3 — the S2M operators against plain PyTorch statements of the same ops
-(tests/abi_emulator.py: F.unfold / F.interpolate / mean on the CPU), and the S2M network and
-controller against the vectors the UNMODIFIED reference produced (tests/golden/s2m_*.npz).
-Gathers and the pooled broadcast of fp16-representable values are bit-exact; bilinear resizes equal
-ATen's to fp32 rounding (1e-6) plus one fp16 rounding for fp16 maps; network outputs carry the conv
-tolerances of DESIGN.md §6 (fp16 / TF32 operands, fp32 accumulation)."""
+"""GPU: the S2M operators (csrc/halo_ops.cu, csrc/elementwise.cu) against plain float64 statements of the same
+operations, and the S2M network and controller against the vectors the UNMODIFIED reference produced
+(tests/golden/s2m_*.npz).
+
+The operator tests follow tests/test_gpu_ops_ragged.py: every reference is computed from the operands the kernel saw
+(fp16-rounded for fp16 maps); the dilated gather is bit-exact; outputs are pre-filled with a sentinel that must
+survive outside the written window; inputs the kernel must not read (HALO borders, channels outside the window) hold
+NaN.  The arithmetic kernels get elementwise bounds derived from their fp32 operations (u = 2^-24), and every check
+prints its largest err/bound ratio (run with -s):
+  * halo_avgpool_broadcast: each of 8 pixel groups sums its pixels sequentially, the 8 partials are added, the sum is
+    multiplied by fl(1/hw): |m - mu| <= ((ceil(hw/8) + 7) u sum|x|) / hw + 2u |mu|;
+  * upsample_bilinear, halo_upsample_to_plane: 5u sum|w v| where the scale in/out is a power of two (exact weights),
+    6u sum|w v| elsewhere (1 - l rounds too), plus dsrc D per axis: fl(in/out) and the source coordinate put the
+    sample at most dsrc <= 3u (in + 1) off, and the interpolant moves by at most D (the largest difference of
+    neighbouring source values along that axis) per unit; through the sigmoid p(1-p) err + p(2u + 4u(1-p));
+  * fp16 maps round the result once more: 2^-11 |ref| (2^-25 absolute below the normal range).
+Network outputs carry the conv tolerances of DESIGN.md §6 (fp16 / TF32 operands, fp32 accumulation)."""
+import math
+
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
-import abi_emulator as E  # noqa: E402
 from mivos_b200 import _lib, ops  # noqa: E402
+from test_gpu_ops_ragged import H16, NAN, SENT, U, VEC, _check, _halo, _round16  # noqa: E402
 
 DT = {"fp16": torch.float16, "tf32": torch.float32}
 
@@ -28,93 +42,157 @@ def _sync():
     _lib.poll_kernel_error()
 
 
-def _rand16(shape, seed):
-    """fp32 values that are exactly representable in fp16 (so copies are exact in both map types)."""
-    g = torch.Generator().manual_seed(seed)
-    return torch.randn(shape, generator=g).half().float()
+def _outside(t, n, h, w, coff, c):
+    """Mask of everything but the interior pixels of channels [coff, coff + c) of a HALO map."""
+    m = torch.ones(t.shape, dtype=torch.bool, device=t.device)
+    m[:, 1:h + 1, 1:w + 1, coff:coff + c] = False
+    return m
 
 
-@pytest.mark.parametrize("act", ["fp16", "tf32"])
-@pytest.mark.parametrize("n,h,w,c,dil", [(1, 6, 8, 64, 2), (2, 30, 54, 128, 6), (1, 30, 54, 64, 18), (1, 9, 7, 32, 12)])
-def test_gather_dilated(dev, act, n, h, w, c, dil):
-    dt = DT[act]
-    x = _rand16((n, c, h, w), 3 * c + dil)
-    xh_cpu = to_halo(x)
-    rows = n * (h + 2) * (w + 2)
-    want = E.gather_dilated(xh_cpu, n, h, w, c, dil, torch.full((rows, 9 * c), 5.0))
-    got = torch.full((rows, 9 * c), 5.0, device=dev, dtype=dt)
-    ops.gather_dilated(to_halo(x.to(dev), dtype=dt), n, h, w, c, dil, got)
+# ------------------------------------------------------------------------------------------ dilated gather
+@pytest.mark.parametrize("dtype", [torch.float32, H16])
+@pytest.mark.parametrize("dil", [1, 2, 6, 12, 18])
+def test_gather_dilated(dev, dtype, dil):
+    """out[r, (ky*3 + kx)*c + ci] = x[y + (ky-1) d, x + (kx-1) d, ci] (zero outside the map): F.unfold(dilation=d,
+    padding=d) reordered to (ky, kx, c).  Three images of different content; a d x d map, where only the centre tap
+    is live; a (2d + 3) x (d + 5) map, on which dilation d + 1 reads other pixels; c of one 16-byte vector and a c
+    that is not a multiple of 32.  The input holds NaN in its border and in one vector of channels past c; the output
+    has one vector of columns past 9c that must keep the sentinel, and its HALO border rows are zero rows."""
+    v = VEC[dtype]
+    g = torch.Generator().manual_seed(dil)
+    for n, h, w, c in ((3, 9, 13, 40 if dtype == torch.float32 else 72), (1, dil, dil, v), (2, 5, 3, v),
+                       (2, 2 * dil + 3, dil + 5, v)):
+        x = torch.randn(n, c, h, w, generator=g).to(dtype).to(dev)
+        src = _halo(x, c + v, fill=NAN, dtype=dtype)
+        got = torch.full((n, h + 2, w + 2, 9 * c + v), SENT, dtype=dtype, device=dev)
+        ops.gather_dilated(src, n, h, w, c, dil, got)
+        _sync()
+        cols = F.unfold(x.double(), 3, dilation=dil, padding=dil)  # [n, c*9, h*w], (c, ky, kx) order
+        cols = cols.reshape(n, c, 9, h, w).permute(0, 3, 4, 2, 1).reshape(n, h, w, 9 * c)
+        exp = torch.full_like(got, SENT)
+        exp[..., :9 * c] = 0
+        exp[:, 1:-1, 1:-1, :9 * c] = cols.to(dtype)
+        assert torch.equal(got, exp), f"gather_dilated d={dil} {n}x{h}x{w} c={c}"
+
+
+# ------------------------------------------------------------------------------------------ pooled broadcast
+def avgpool_reference(x):
+    """fp64 mean over the pixels of x [n, c, h, w] and its bound for the kernel's summation order (module docstring)."""
+    n, c, h, w = x.shape
+    hw = h * w
+    xd = x.double()
+    mu = xd.mean((2, 3))
+    s = xd.abs().sum((2, 3))
+    return mu, (math.ceil(hw / 8) + 7) * U * s / hw + 2 * U * mu.abs()
+
+
+# (n, h, w, c, in_coff, out_coff, spread of the per-image offsets, common offset)
+AVGPOOL_CASES = [
+    (2, 1, 1, None, 0, 0, 0.0, 0.0),      # hw = 1
+    (1, 1, 5, None, 0, 0, 0.0, 0.0),      # hw = 5: three of the 8 pixel groups idle
+    (1, 45, 80, None, 0, 0, 0.0, 0.0),    # the 1/16 map of 720p: 3600 pixels
+    (1, 6, 8, 2048, 1, 2, 0.0, 0.0),      # the 2048-channel ASPP input, both channel windows offset (in vectors)
+    (3, 5, 7, None, 1, 0, 10.0, 0.0),     # per-image offsets: mixing images shows
+    (1, 9, 13, None, 0, 1, 0.0, 1000.0),  # mean 1000, spread 1
+]
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, H16])
+@pytest.mark.parametrize("case", range(len(AVGPOOL_CASES)))
+def test_avgpool_broadcast(dev, dtype, case):
+    n, h, w, c, in_v, out_v, spread, offset = AVGPOOL_CASES[case]
+    v = VEC[dtype]
+    c = c or (40 if dtype == torch.float32 else 8)  # 10 vectors / 1 vector: neither fills the 32 lanes of a CTA
+    in_coff, out_coff = in_v * v, out_v * v
+    g = torch.Generator().manual_seed(case)
+    base = offset + spread * torch.arange(n, dtype=torch.float32).reshape(n, 1, 1, 1)
+    x = (torch.randn(n, c, h, w, generator=g) + base).to(dtype).to(dev)
+    src = _halo(x, in_coff + c + v, in_coff, fill=NAN, dtype=dtype)
+    out = torch.full((n, h + 2, w + 2, out_coff + c + v), SENT, dtype=dtype, device=dev)
+    ops.halo_avgpool_broadcast(src, n, h, w, c, out, in_coff=in_coff, out_coff=out_coff)
     _sync()
-    assert torch.equal(got.float().cpu(), want)
+    mu, bound = avgpool_reference(x)
+    win = out[:, 1:-1, 1:-1, out_coff:out_coff + c]
+    assert bool((win == win[:, :1, :1]).all()), "the mean is not the same at every pixel"
+    _check(f"avgpool {dtype} n={n} {h}x{w} c={c}", win[:, 0, 0], mu, _round16(bound, mu, dtype))
+    assert bool((out[_outside(out, n, h, w, out_coff, c)] == SENT).all()), "written outside the window"
 
 
-@pytest.mark.parametrize("act", ["fp16", "tf32"])
-def test_stem_gather_six_channels(dev, act):
-    dt = DT[act]
-    n, h, w = 2, 32, 48
-    x = _rand16((n, 6, h, w), 17)
-    rows = n * (h // 2 + 2) * (w // 2 + 2)
-    want = E.stem_gather_frames(x, torch.zeros((rows, 320)))
-    got = torch.full((rows, 320), 3.0, device=dev, dtype=dt)
-    ops.stem_gather_frames(x.to(dev), got)
+# ------------------------------------------------------------------------------------------ bilinear resizes
+def bilinear_reference(x, h, w):
+    """fp64 F.interpolate(size=(h, w), align_corners=False) of x [n, c, hs, ws] and the kernels' bound on it
+    (module docstring)."""
+    hs, ws = x.shape[-2:]
+    xd = x.double()
+    ref = F.interpolate(xd, size=(h, w), mode="bilinear", align_corners=False)
+    mag = F.interpolate(xd.abs(), size=(h, w), mode="bilinear", align_corners=False)
+    exact = all(math.log2(a / b).is_integer() for a, b in ((hs, h), (ws, w)))
+    bound = (5 if exact else 6) * U * mag
+    if not exact:
+        dy = float(xd.diff(dim=2).abs().max()) if hs > 1 else 0.0
+        dx = float(xd.diff(dim=3).abs().max()) if ws > 1 else 0.0
+        bound = bound + 3 * U * (hs + 1) * dy + 3 * U * (ws + 1) * dx
+    return ref, bound
+
+
+# (n, hs, ws, h, w, c (None: a ragged count), src_coff, dst_coff)
+RESIZE_CASES = [
+    (1, 45, 80, 180, 320, 256, 1, 48),  # x4, the S2M head at 720p: ASPP output into the 304-channel concat map
+    (2, 7, 5, 10, 13, None, 0, 0),
+    (1, 13, 9, 5, 4, None, 1, 2),       # downsampling
+    (3, 1, 1, 6, 8, None, 0, 1),
+    (1, 6, 8, 1, 1, None, 2, 0),
+]
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, H16])
+@pytest.mark.parametrize("case", range(len(RESIZE_CASES)))
+def test_upsample_bilinear_window(dev, dtype, case):
+    n, hs, ws, h, w, c, s_v, d_v = RESIZE_CASES[case]
+    v = VEC[dtype]
+    c = c or (40 if dtype == torch.float32 else 72)
+    s_coff = s_v * v
+    d_coff = 48 if d_v == 48 else d_v * v
+    x = (torch.randn(n, c, hs, ws, generator=torch.Generator().manual_seed(case)) * 3).to(dtype).to(dev)
+    src = _halo(x, s_coff + c + v, s_coff, fill=NAN, dtype=dtype)
+    out = torch.full((n, h + 2, w + 2, d_coff + c + v), SENT, dtype=dtype, device=dev)
+    ops.upsample_bilinear(src, n, hs, ws, out, h, w, c, src_coff=s_coff, dst_coff=d_coff)
     _sync()
-    assert torch.equal(got.float().cpu(), want)
-    # the 3-channel entry is the batch form of mivos_stem_gather
-    x3 = _rand16((n, 3, h, w), 18)
-    kp = 192 if act == "fp16" else 160
-    a = torch.zeros((rows, kp), device=dev, dtype=dt)
-    b = torch.zeros((rows, kp), device=dev, dtype=dt)
-    ops.stem_gather_frames(x3.to(dev), a)
-    ops.stem_gather(x3.to(dev), None, b)
-    _sync()
-    assert torch.equal(a, b)
+    ref, bound = bilinear_reference(x, h, w)
+    got = out[:, 1:-1, 1:-1, d_coff:d_coff + c].permute(0, 3, 1, 2)
+    _check(f"upsample_bilinear {dtype} {hs}x{ws}->{h}x{w} c={c}", got, ref, _round16(bound, ref, dtype))
+    assert bool((out[_outside(out, n, h, w, d_coff, c)] == SENT).all()), "written outside the window"
 
 
-@pytest.mark.parametrize("act", ["fp16", "tf32"])
-@pytest.mark.parametrize("n,h,w,c", [(1, 6, 8, 2048), (3, 30, 54, 256), (1, 5, 3, 40)])
-def test_avgpool_broadcast(dev, act, n, h, w, c):
-    dt = DT[act]
-    x = _rand16((n, c, h, w), c + h)
-    cs = c + 24
-    want = E.halo_avgpool_broadcast(to_halo(x, cs), n, h, w, c, torch.zeros((n, h + 2, w + 2, cs + 8)), in_coff=0, out_coff=8)
-    src = torch.zeros((n, h + 2, w + 2, cs), device=dev, dtype=dt)
-    src[:, 1:-1, 1:-1, 16:16 + c] = x.permute(0, 2, 3, 1).to(dev)
-    got = torch.zeros((n, h + 2, w + 2, cs + 8), device=dev, dtype=dt)
-    ops.halo_avgpool_broadcast(src, n, h, w, c, got, in_coff=16, out_coff=8)
-    _sync()
-    tol = 1e-3 if act == "fp16" else 1e-6  # fp32 sum in another order (+ one fp16 rounding of the mean)
-    assert float((got.float().cpu() - want).abs().max()) <= tol
-    assert float(got[:, 0].abs().max()) == 0 and float(got[:, :, -1].abs().max()) == 0  # border untouched
-    assert float(got[..., :8].abs().max()) == 0 and float(got[..., 8 + c:].abs().max()) == 0  # window only
-
-
-@pytest.mark.parametrize("act", ["fp16", "tf32"])
-@pytest.mark.parametrize("n,hs,ws,h,w,c", [(1, 6, 8, 24, 32, 256), (2, 30, 54, 120, 216, 64), (1, 1, 1, 6, 8, 32),
-                                           (1, 7, 5, 10, 13, 16)])
-def test_upsample_bilinear_window(dev, act, n, hs, ws, h, w, c):
-    dt = DT[act]
-    x = _rand16((n, c, hs, ws), hs * 5 + c)
-    want = E.upsample_bilinear(to_halo(x), n, hs, ws, torch.zeros((n, h + 2, w + 2, c + 64)), h, w, c, dst_coff=48)
-    got = torch.zeros((n, h + 2, w + 2, c + 64), device=dev, dtype=dt)
-    ops.upsample_bilinear(to_halo(x.to(dev), dtype=dt), n, hs, ws, got, h, w, c, dst_coff=48)
-    _sync()
-    tol = 4e-3 if act == "fp16" else 2e-6  # values up to ~4: half an fp16 ulp is 2e-3
-    assert float((got.float().cpu() - want).abs().max()) <= tol
-    assert float(got[:, 0].abs().max()) == 0 and float(got[:, :, 0].abs().max()) == 0
-    assert float(got[..., :48].abs().max()) == 0 and float(got[..., 48 + c:].abs().max()) == 0
+PLANE_CASES = [
+    (1, 180, 320, 720, 1280),  # x4, the S2M output at 720p
+    (2, 7, 5, 10, 13),
+    (1, 13, 9, 5, 4),
+    (1, 1, 1, 6, 8),
+    (1, 6, 8, 1, 1),
+]
 
 
 @pytest.mark.parametrize("sig", [False, True])
-@pytest.mark.parametrize("n,hs,ws,H,W", [(1, 24, 32, 96, 128), (3, 120, 216, 480, 864), (2, 5, 7, 13, 9)])
-def test_upsample_to_plane(dev, sig, n, hs, ws, H, W):
-    x = torch.randn((n, 1, hs, ws), generator=torch.Generator().manual_seed(hs)) * 3
-    hb = torch.zeros((n, hs + 2, ws + 2, 32))
-    hb[:, 1:-1, 1:-1, 4:5] = x.permute(0, 2, 3, 1)
-    want = E.halo_upsample_to_plane(hb, n, hs, ws, H, W, coff=4, sigmoid=sig)
-    got = ops.halo_upsample_to_plane(hb.to(dev), n, hs, ws, H, W, coff=4, sigmoid=sig)
+@pytest.mark.parametrize("case", range(len(PLANE_CASES)))
+def test_upsample_to_plane(dev, sig, case):
+    """One channel (5 of 7; NaN in the others and the border) of an fp32 HALO map -> NCHW planes.  A quarter of the
+    logits sit at +-30, where the sigmoid saturates.  One element past the planes must keep the sentinel."""
+    n, hs, ws, H, W = PLANE_CASES[case]
+    g = torch.Generator().manual_seed(100 + case)
+    x = torch.randn(n, 1, hs, ws, generator=g) * 3
+    pick = torch.randint(0, 8, x.shape, generator=g)
+    x = torch.where(pick == 0, torch.full_like(x, 30.0), torch.where(pick == 1, torch.full_like(x, -30.0), x)).to(dev)
+    halo = _halo(x, 7, 5, fill=NAN)
+    buf = torch.full((n * H * W + 1,), SENT, device=dev)
+    got = ops.halo_upsample_to_plane(halo, n, hs, ws, H, W, coff=5, sigmoid=sig, out=buf[:-1].view(n, 1, H, W))
     _sync()
-    assert got.shape == (n, 1, H, W)
-    assert float((got.cpu() - want).abs().max()) <= 1e-5
+    assert float(buf[-1]) == SENT
+    ref, bound = bilinear_reference(x, H, W)
+    if sig:
+        p = torch.sigmoid(ref)
+        ref, bound = p, p * (1 - p) * bound + p * (2 * U + 4 * U * (1 - p))
+    _check(f"upsample_to_plane {hs}x{ws}->{H}x{W} sigmoid={sig}", got, ref, bound)
 
 
 @pytest.mark.parametrize("act", ["fp16", "tf32"])
