@@ -264,6 +264,19 @@ MIVOS_API int mivos_attention_map(const float* mk, const float* qk, int h16, int
  * fp32 row-major.  mk, qk pixel-major [hw][128]; scratch: 4*hw floats.                            */
 MIVOS_API int mivos_attention_weights(const float* mk, const float* qk, int hw, float* w_out, float* scratch,
                             mivos_stream_t stream);
+/* Whether mivos_attention_map / mivos_attention_weights take hw key pixels: *resident = 1 when one logit row per
+ * query of the CTA fits their shared-memory tile (hw <= 6912), 0 otherwise.  Pure host arithmetic, no device.     */
+MIVOS_API int mivos_attention_plan(int hw, int* resident);
+/* The same two operators for ANY hw >= 1 (a 1080p frame pads to 68 x 120 = 8160 key pixels, 4K to 135 x 240):
+ * prop_net.py:115-129,187-200 (get_attention) and prop_net.py:183 (get_W), same arguments, layouts and scratch
+ * (4*hw floats) as mivos_attention_map / mivos_attention_weights.  The memory keys are streamed through shared
+ * memory in tiles and the softmax over the memory axis is computed online (running maximum, partial sums
+ * rescaled when it grows); the logits are the same fp32 fma chains as the resident kernel's.  The weights form
+ * makes one such pass for the column maximum and denominator, then writes w_out row by row.                    */
+MIVOS_API int mivos_attention_map_streamed(const float* mk, const float* qk, int h16, int w16, const float* pos,
+                                 const float* neg, float* out, float* scratch, mivos_stream_t stream);
+MIVOS_API int mivos_attention_weights_streamed(const float* mk, const float* qk, int hw, float* w_out,
+                                     float* scratch, mivos_stream_t stream);
 /* FusionNet input gather (fusion_net.py:35-40): cat(im, seg1, seg2, attn, time) -> HALO
  * (1, H, W, cpad) with channels 9..cpad-1 zero.                                                 */
 MIVOS_API int mivos_fusion_gather(const float* im, const float* seg1, const float* seg2, const float* attn,
@@ -280,6 +293,14 @@ MIVOS_API int mivos_halo_sigmoid_to_plane(const float* halo, int h, int w, int c
  * davis_processor.py:66 / interact/s2m_controller.py:34).  Output as mivos_stem_gather.          */
 MIVOS_API int mivos_stem_gather_frames(const float* frames, int n, int cin, int h, int w, void* out, int kpad,
                              int out_f16, mivos_stream_t stream);
+/* Whether mivos_stem_gather_frames takes cin-channel frames w pixels wide: *untiled = 1 when 7 whole input rows
+ * fit its shared memory (cin 6: w <= 1376 in fp32, w <= 2760 in fp16), 0 otherwise.  Pure host arithmetic.       */
+MIVOS_API int mivos_stem_frames_plan(int cin, int w, int out_f16, int* untiled);
+/* mivos_stem_gather_frames for the 6-channel S2M stem (s2m_resnet.py:93-94) at ANY frame width: the output row
+ * is gathered in windows of output columns, each staging only the input columns it reads (zero padding at the
+ * image edges only).  Same output matrix as mivos_stem_gather_frames, bit for bit.                              */
+MIVOS_API int mivos_stem_gather_frames_tiled(const float* frames, int n, int h, int w, void* out, int kpad,
+                                   int out_f16, mivos_stream_t stream);
 /* Dilated 3x3/stride-1/pad=dilation gather from a HALO map into an im2col matrix whose rows are
  * the HALO rows of the output map: out[r, (ky*3+kx)*c + ci] (s2m_resnet.py:19-20 conv3x3 with
  * dilation 2 in layer4; _deeplab.py:119-124 ASPPConv with rates 6/12/18).                        */

@@ -91,9 +91,14 @@ SIGNATURES = {
     "mivos_pad2d": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _p, _p]),
     "mivos_attention_map": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _p]),
     "mivos_attention_weights": (_i, [_p, _p, _i, _p, _p, _p]),
+    "mivos_attention_plan": (_i, [_i, C.POINTER(_i)]),
+    "mivos_attention_map_streamed": (_i, [_p, _p, _i, _i, _p, _p, _p, _p, _p]),
+    "mivos_attention_weights_streamed": (_i, [_p, _p, _i, _p, _p, _p]),
     "mivos_fusion_gather": (_i, [_p, _p, _p, _p, _f, _f, _i, _i, _p, _i, _i, _p]),
     "mivos_halo_sigmoid_to_plane": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "mivos_stem_gather_frames": (_i, [_p, _i, _i, _i, _i, _p, _i, _i, _p]),
+    "mivos_stem_frames_plan": (_i, [_i, _i, _i, C.POINTER(_i)]),
+    "mivos_stem_gather_frames_tiled": (_i, [_p, _i, _i, _i, _p, _i, _i, _p]),
     "mivos_gather_dilated": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _p]),
     "mivos_halo_avgpool_broadcast": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p]),
     "mivos_upsample_bilinear": (_i, [_p, _i, _i, _i, _i, _i, _p, _i, _i, _i, _i, _i, _i, _p]),

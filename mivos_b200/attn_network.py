@@ -9,7 +9,7 @@ objects' mask differences into attention maps.  Same sub-module names as the pro
 Runs on the kernels of the propagation path: the 5-channel memory encoder with K = 2 objects
 (each object's "other" mask is the second object's mask, attn_network.py:60-61), the query encoder,
 and mivos_attention_map (softmax over the memory axis, area pooling, row-vector product, bilinear
-resize) — W [HW, HW] never leaves shared memory.
+resize; mivos_attention_map_streamed above 6912 key pixels) — W [HW, HW] is never written to memory.
 """
 from __future__ import annotations
 
@@ -77,11 +77,12 @@ class AttentionReadNetwork(nn.Module):
         out2 = torch.empty_like(out1)
         mk = torch.empty((2, h * w, 128), dtype=torch.float32, device=image.device)
         qs = None
+        attention_map = ops.attention_op(h * w)
         for i in range(b):
             # objects (mask21, other = mask22) and (mask22, other = mask21): one K = 2 memory pass (:59-60)
             kv = eng.encode_memory(image[i:i + 1], torch.cat([m21[i:i + 1], m22[i:i + 1]], 0))
             ops.halo_to_pixels(kv, 2, h, w, 0, 128, mk)
             qs = eng.encode_query(query_image[i:i + 1], qs)  # :62-63
-            out1[i:i + 1] = ops.attention_map(mk[0], qs.qk, h, w, pos1[i:i + 1].contiguous(), neg1[i:i + 1].contiguous())
-            out2[i:i + 1] = ops.attention_map(mk[1], qs.qk, h, w, pos2[i:i + 1].contiguous(), neg2[i:i + 1].contiguous())
+            out1[i:i + 1] = attention_map(mk[0], qs.qk, h, w, pos1[i:i + 1].contiguous(), neg1[i:i + 1].contiguous())
+            out2[i:i + 1] = attention_map(mk[1], qs.qk, h, w, pos2[i:i + 1].contiguous(), neg2[i:i + 1].contiguous())
         return out1, out2

@@ -8,6 +8,7 @@
 
 #include <atomic>
 #include <cuda_fp16.h>
+#include <mutex>
 
 namespace mivos {
 extern std::atomic<int64_t> g_launches;
@@ -92,12 +93,17 @@ constexpr int kStemThreads = 512;
 template <int CIN, typename T>
 __global__ void __launch_bounds__(kStemThreads)
 stem_gather_kernel(const float* __restrict__ frame, const float* __restrict__ masks, int kobj, int h, int w,
-                   T* __restrict__ out, int kpad, int64_t frame_gstride, int64_t mask_gstride) {
+                   T* __restrict__ out, int kpad, int64_t frame_gstride, int64_t mask_gstride, int wcols) {
   mivos::pdl_prologue();
   extern __shared__ __align__(16) uint8_t stem_smem[];
-  T* win = reinterpret_cast<T*>(stem_smem);  // [7][w + 6][CIN]
   const int ho = h / 2, wo = w / 2;
   const int wp = wo + 2;
+  // column window: output columns [xo0, xo0 + nwo) of the frame (one window of wcols = wo: the whole row); the HALO
+  // pad columns belong to the first and the last window
+  const int xo0 = static_cast<int>(blockIdx.z) * wcols;
+  const int nwo = wo - xo0 < wcols ? wo - xo0 : wcols;
+  const int sw = 2 * nwo + 6;                // staged pixels per row: input x = 2 xo0 - 3 + xs
+  T* win = reinterpret_cast<T*>(stem_smem);  // [7][sw][CIN]
   const int yo = static_cast<int>(blockIdx.x) - 1;  // output row, -1 and ho are halo rows
   const int img = blockIdx.y;                       // output image: group (clip) major
   // CIN == 5: image = object `obj` of group `img / kobj` (own frame, own K masks); otherwise a batch of frames
@@ -107,7 +113,7 @@ stem_gather_kernel(const float* __restrict__ frame, const float* __restrict__ ma
     masks += static_cast<int64_t>(img / kobj) * mask_gstride;
   }
   const int64_t plane = static_cast<int64_t>(h) * w;
-  const int rowlen = (w + 6) * CIN;
+  const int rowlen = sw * CIN;
   const bool live_row = yo >= 0 && yo < ho;
 
   if (live_row) {
@@ -117,9 +123,9 @@ stem_gather_kernel(const float* __restrict__ frame, const float* __restrict__ ma
     const float* fr = frame + (CIN == 5 ? 0 : static_cast<int64_t>(obj) * CIN * plane);
     // (latency-bound: ~12 staged pixels per thread, 3-5 independent global loads each)
 #pragma unroll 4
-    for (int i = threadIdx.x; i < 7 * (w + 6); i += kStemThreads) {
-      const int ky = i / (w + 6), xs = i - ky * (w + 6);
-      const int y = 2 * yo + ky - 3, x = xs - 3;
+    for (int i = threadIdx.x; i < 7 * sw; i += kStemThreads) {
+      const int ky = i / sw, xs = i - ky * sw;
+      const int y = 2 * yo + ky - 3, x = 2 * xo0 + xs - 3;
       float v[CIN];
 #pragma unroll
       for (int c = 0; c < CIN; ++c) v[c] = 0.f;
@@ -139,7 +145,7 @@ stem_gather_kernel(const float* __restrict__ frame, const float* __restrict__ ma
         }
       }
 #pragma unroll
-      for (int c = 0; c < CIN; ++c) win[(ky * (w + 6) + xs) * CIN + c] = from_float<T>(v[c]);
+      for (int c = 0; c < CIN; ++c) win[(ky * sw + xs) * CIN + c] = from_float<T>(v[c]);
     }
   }
   __syncthreads();
@@ -149,11 +155,12 @@ stem_gather_kernel(const float* __restrict__ frame, const float* __restrict__ ma
   constexpr int RUN = 7 * CIN;  // contiguous elements of one window row
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int64_t row_base = (static_cast<int64_t>(img) * (ho + 2) + yo + 1) * wp;
-  for (int xp = warp; xp < wp; xp += nwarps) {
+  const int xp_end = xo0 + nwo == wo ? wp : xo0 + nwo + 1;
+  for (int xp = (xo0 == 0 ? 0 : xo0 + 1) + warp; xp < xp_end; xp += nwarps) {
     const int xo = xp - 1;
     const bool live = live_row && xo >= 0 && xo < wo;
     T* orow = out + (row_base + xp) * kpad;
-    const T* src = win + 2 * xo * CIN;  // window starts at input x = 2 xo - 3, i.e. staged x = 2 xo
+    const T* src = win + 2 * (xo - xo0) * CIN;  // window starts at input x = 2 xo - 3, i.e. staged x = 2 (xo - xo0)
     for (int k0 = lane * V; k0 < kpad; k0 += 32 * V) {
       alignas(16) T vals[V];
 #pragma unroll
@@ -165,6 +172,27 @@ stem_gather_kernel(const float* __restrict__ frame, const float* __restrict__ ma
       *reinterpret_cast<uint4*>(orow + k0) = *reinterpret_cast<const uint4*>(vals);
     }
   }
+}
+
+// Staged rows of one launch of stem_gather_kernel: 7 rows of (2 * wcols + 6) pixels x CIN channels.  The untiled
+// entry points stage whole rows (wcols = w / 2) and refuse frames whose rows do not fit the opt-in limit.
+constexpr int kMaxStemSmem = 227 * 1024;
+inline int64_t stem_rows_smem(int cin, int wcols, int f16) { return 7ll * (2ll * wcols + 6) * cin * (f16 ? 2 : 4); }
+// Output columns per window of mivos_stem_gather_frames_tiled: 7 x 262 pixels x 6 channels x 4 B = 44 KB of staged
+// rows at any frame width.
+constexpr int kStemWindow = 128;
+
+// The opt-in shared-memory limit of one stem_gather_kernel instance, shared by the entry points that launch it: only
+// ever raised (lowering it would make a later launch that had been allowed fail).
+template <int CIN, typename T>
+cudaError_t reserve_stem_smem(int smem) {
+  static std::mutex mu;
+  static int configured = 0;
+  std::lock_guard<std::mutex> lock(mu);
+  if (smem <= configured) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(stem_gather_kernel<CIN, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e == cudaSuccess) configured = smem;
+  return e;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -617,17 +645,14 @@ extern "C" MIVOS_API int mivos_stem_gather(const float* frame, const float* mask
   MIVOS_REQUIRE(kpad >= 49 * cin && kpad % 32 == 0, "stem_gather: kpad %d too small for cin %d", kpad, cin);
   MIVOS_REQUIRE(kpad % 8 == 0 && AL16(out), "stem_gather: output rows must be 16-byte aligned");
   const dim3 grid(h / 2 + 2, k_objects * groups);
-  const int smem = 7 * (w + 6) * cin * (out_f16 ? 2 : 4);
-  MIVOS_REQUIRE(smem <= 227 * 1024, "stem_gather: a %d-pixel wide frame needs %d B of shared memory", w, smem);
+  const int smem = static_cast<int>(stem_rows_smem(cin, w / 2, out_f16));
+  MIVOS_REQUIRE(smem <= kMaxStemSmem, "stem_gather: a %d-pixel wide frame needs %d B of shared memory", w, smem);
+  const int wcols = w / 2;
 #define STEM(CIN_, T_)                                                                                          \
   do {                                                                                                          \
-    static int configured = 0;                                                                                  \
-    if (smem > configured) {                                                                                    \
-      MIVOS_CUDA_OK(cudaFuncSetAttribute(stem_gather_kernel<CIN_, T_>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-      configured = smem;                                                                                        \
-    }                                                                                                           \
+    MIVOS_CUDA_OK((reserve_stem_smem<CIN_, T_>(smem)));                                                         \
     launch_pdl(stem_gather_kernel<CIN_, T_>, grid, kStemThreads, smem, ST(s), frame, masks, k_objects, h, w,    \
-               static_cast<T_*>(out), kpad, frame_gstride, mask_gstride);                                       \
+               static_cast<T_*>(out), kpad, frame_gstride, mask_gstride, wcols);                                \
   } while (0)
   if (out_f16) {
     if (masks) STEM(5, __half);
@@ -686,8 +711,36 @@ extern "C" MIVOS_API int mivos_stem_gather_frames(const float* frames, int n, in
   const int k_objects = n;
   const int64_t frame_gstride = 0, mask_gstride = 0;
   const dim3 grid(h / 2 + 2, n);
-  const int smem = 7 * (w + 6) * cin * (out_f16 ? 2 : 4);
-  MIVOS_REQUIRE(smem <= 227 * 1024, "stem_gather_frames: a %d-pixel wide frame needs %d B of shared memory", w, smem);
+  const int smem = static_cast<int>(stem_rows_smem(cin, w / 2, out_f16));
+  MIVOS_REQUIRE(smem <= kMaxStemSmem, "stem_gather_frames: a %d-pixel wide frame needs %d B of shared memory", w, smem);
+  const int wcols = w / 2;
+  if (out_f16) STEM(6, __half);
+  else STEM(6, float);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_stem_frames_plan(int cin, int w, int out_f16, int* untiled) {
+  MIVOS_REQUIRE(untiled, "stem_frames_plan: null pointer");
+  MIVOS_REQUIRE(cin == 3 || cin == 6, "stem_frames_plan: %d input channels (3 or 6)", cin);
+  MIVOS_REQUIRE(w > 0 && w % 2 == 0, "stem_frames_plan: bad width %d", w);
+  *untiled = stem_rows_smem(cin, w / 2, out_f16) <= kMaxStemSmem ? 1 : 0;
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_stem_gather_frames_tiled(const float* frames, int n, int h, int w, void* out, int kpad,
+                                                        int out_f16, mivos_stream_t s) {
+  MIVOS_REQUIRE(frames && out, "stem_gather_frames_tiled: null pointer");
+  MIVOS_REQUIRE(h % 2 == 0 && w % 2 == 0 && h > 0 && w > 0 && n >= 1, "stem_gather_frames_tiled: bad shape");
+  MIVOS_REQUIRE(kpad >= 49 * 6 && kpad % 32 == 0 && AL16(out), "stem_gather_frames_tiled: kpad %d too small / unaligned", kpad);
+  MIVOS_REQUIRE(n <= 65535, "stem_gather_frames_tiled: %d frames", n);
+  const float* frame = frames;
+  const float* masks = nullptr;
+  const int k_objects = n;
+  const int64_t frame_gstride = 0, mask_gstride = 0;
+  const int wcols = w / 2 < kStemWindow ? w / 2 : kStemWindow;
+  const dim3 grid(h / 2 + 2, n, ceil_div(w / 2, wcols));
+  const int smem = static_cast<int>(stem_rows_smem(6, wcols, out_f16));
   if (out_f16) STEM(6, __half);
   else STEM(6, float);
   MIVOS_LAUNCHED();

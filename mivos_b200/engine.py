@@ -519,7 +519,10 @@ class S2MEngine(_ResNetTrunk):
         assert cin == 6 and H % 16 == 0 and W % 16 == 0, "S2M input: [n,6,H,W], H and W multiples of 16 (pad_divide_by)"
         ws, pc = self.ws, self.pc
         stem = ws.mat("stem", n * (H // 2 + 2) * (W // 2 + 2), pc["backbone.conv1"].cin_pad)
-        ops.stem_gather_frames(x, stem)
+        if ops.stem_frames_untiled(cin, W, stem.dtype == torch.float16):
+            ops.stem_gather_frames(x, stem)
+        else:  # wider than 7 staged input rows fit in shared memory: 1378 px in fp32, 2762 in fp16
+            ops.stem_gather_frames_tiled(x, stem)
         h4, w4, h16, w16 = H // 4, W // 4, H // 16, W // 16
         low = ws.halo("low", n, h4, w4, 256)
         f = self._trunk("backbone", arch.S2M_LAYERS, stem, n, H, W, {0: low}, ws, planes_t=arch.S2M_PLANES,

@@ -457,6 +457,55 @@ def attention_weights(mk: torch.Tensor, qk: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def _attention_operands(mk: torch.Tensor, qk: torch.Tensor, what: str) -> int:
+    _req(mk), _req(qk)
+    if mk.dim() != 2 or mk.shape[1] != 128 or qk.shape != mk.shape:
+        raise _lib.MivosError(f"{what}: mk {tuple(mk.shape)} / qk {tuple(qk.shape)} are not both [hw,128]")
+    return mk.shape[0]
+
+
+def attention_map_streamed(mk: torch.Tensor, qk: torch.Tensor, h16: int, w16: int, pos: torch.Tensor,
+                           neg: torch.Tensor) -> torch.Tensor:
+    """attention_map for any number of key pixels (mivos_attention_map_streamed)."""
+    if _attention_operands(mk, qk, "attention_map_streamed") != h16 * w16:
+        raise _lib.MivosError(f"attention_map_streamed: mk {tuple(mk.shape)} is not [{h16 * w16},128]")
+    _req(pos), _req(neg)
+    for t in (pos, neg):
+        if tuple(t.shape) != (1, 1, 16 * h16, 16 * w16):
+            raise _lib.MivosError(f"attention_map_streamed: pos/neg {tuple(t.shape)} are not [1,1,{16 * h16},{16 * w16}]")
+    out = torch.empty((1, 2, h16 * 16, w16 * 16), dtype=torch.float32, device=mk.device)
+    scratch = torch.empty(4 * h16 * w16, dtype=torch.float32, device=mk.device)
+    check(_lib.lib().mivos_attention_map_streamed(_ptr(mk), _ptr(qk), h16, w16, _ptr(pos), _ptr(neg), _ptr(out),
+                                                  _ptr(scratch), _stream()), "mivos_attention_map_streamed")
+    return out
+
+
+def attention_weights_streamed(mk: torch.Tensor, qk: torch.Tensor) -> torch.Tensor:
+    """attention_weights for any number of key pixels (mivos_attention_weights_streamed)."""
+    hw = _attention_operands(mk, qk, "attention_weights_streamed")
+    out = torch.empty((hw, hw), dtype=torch.float32, device=mk.device)
+    scratch = torch.empty(4 * hw, dtype=torch.float32, device=mk.device)
+    check(_lib.lib().mivos_attention_weights_streamed(_ptr(mk), _ptr(qk), hw, _ptr(out), _ptr(scratch), _stream()),
+          "mivos_attention_weights_streamed")
+    return out
+
+
+def attention_resident(hw: int) -> bool:
+    """True when the resident attention kernel takes hw key pixels (mivos_attention_plan; no device needed)."""
+    r = C.c_int(0)
+    check(_lib.load().mivos_attention_plan(hw, C.byref(r)), "mivos_attention_plan")
+    return bool(r.value)
+
+
+def attention_op(hw: int, weights: bool = False):
+    """The operator for get_attention (weights=False) or get_W (True) at hw key pixels: attention_map /
+    attention_weights wherever the resident kernel takes the shape — every size it took keeps its results bit for
+    bit —, the streamed form above it (1080p and larger frames)."""
+    if attention_resident(hw):
+        return attention_weights if weights else attention_map
+    return attention_weights_streamed if weights else attention_map_streamed
+
+
 def fusion_gather(im, seg1, seg2, attn, nc: float, nr: float, out_halo: torch.Tensor) -> torch.Tensor:
     for t in (im, seg1, seg2, attn):
         _req(t)
@@ -484,6 +533,24 @@ def stem_gather_frames(frames: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     check(_lib.lib().mivos_stem_gather_frames(_ptr(frames), n, cin, h, w, _ptr(out), out.shape[-1], _f16(out), _stream()),
           "mivos_stem_gather_frames")
     return out
+
+
+def stem_gather_frames_tiled(frames: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """stem_gather_frames for 6-channel frames of any width, gathered in column windows (same matrix, bit for bit)."""
+    _req(frames), _req_act(out)
+    n, cin, h, w = frames.shape
+    if cin != 6:
+        raise _lib.MivosError(f"stem_gather_frames_tiled: {cin} input channels (6)")
+    check(_lib.lib().mivos_stem_gather_frames_tiled(_ptr(frames), n, h, w, _ptr(out), out.shape[-1], _f16(out), _stream()),
+          "mivos_stem_gather_frames_tiled")
+    return out
+
+
+def stem_frames_untiled(cin: int, w: int, f16: bool) -> bool:
+    """True when stem_gather_frames takes cin-channel frames w pixels wide (mivos_stem_frames_plan; no device)."""
+    r = C.c_int(0)
+    check(_lib.load().mivos_stem_frames_plan(cin, w, int(f16), C.byref(r)), "mivos_stem_frames_plan")
+    return bool(r.value)
 
 
 def gather_dilated(x: torch.Tensor, n: int, h: int, w: int, c: int, dilation: int, out: torch.Tensor) -> torch.Tensor:

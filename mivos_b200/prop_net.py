@@ -173,7 +173,8 @@ class PropagationNetwork(nn.Module):
         h, w = qk.shape[-2:]
         hw = h * w
         qpm = qk.reshape(128, hw).t().contiguous()
-        return torch.stack([ops.attention_weights(mk16[i].reshape(128, hw).t().contiguous(), qpm) for i in range(b)], 0)
+        op = ops.attention_op(hw, weights=True)
+        return torch.stack([op(mk16[i].reshape(128, hw).t().contiguous(), qpm) for i in range(b)], 0)
 
     def get_attention(self, mk16, pos_mask, neg_mask, qk16) -> torch.Tensor:
         """prop_net.py:187-200 -> [b,2,H,W] (b = 1 object per call, as in inference_core.py:212)."""
@@ -183,14 +184,16 @@ class PropagationNetwork(nn.Module):
         hw = h * w
         outs = []
         qpm = qk16.reshape(128, hw).t().contiguous()
+        op = ops.attention_op(hw)
         for i in range(b):
             mpm = mk16[i].reshape(128, hw).t().contiguous()
-            outs.append(ops.attention_map(mpm, qpm, h, w, self._f32(pos_mask[i:i + 1]), self._f32(neg_mask[i:i + 1])))
+            outs.append(op(mpm, qpm, h, w, self._f32(pos_mask[i:i + 1]), self._f32(neg_mask[i:i + 1])))
         return outs[0] if b == 1 else torch.cat(outs, 0)
 
     def get_attention_resident(self, mk_pix: torch.Tensor, qs: QueryState, pos_mask, neg_mask) -> torch.Tensor:
         """Same as get_attention with the memory key already pixel-major [hw,128]."""
-        return ops.attention_map(mk_pix, qs.qk, qs.h // 16, qs.w // 16, self._f32(pos_mask), self._f32(neg_mask))
+        h, w = qs.h // 16, qs.w // 16
+        return ops.attention_op(h * w)(mk_pix, qs.qk, h, w, self._f32(pos_mask), self._f32(neg_mask))
 
     def forward(self, *a, **k):  # the reference module has no forward either
         raise NotImplementedError("use memorize / get_query_values / segment_with_query / get_attention")
