@@ -12,13 +12,14 @@
 // under split-K):
 //   warpgroup 0 : one thread is the TMA producer - per (tap, 128-byte k-block) it loads the A box
 //                 {k-block x 128 rows} at the shifted row and the B box {k-block x BN rows} of the
-//                 packed weights, 128B-swizzled, into a ring of STAGES stages
+//                 packed weights, 128B-swizzled, into a ring of STAGES stages; warp 1 bulk-loads
+//                 the residual's interior row segments into the staging tile (SmemLayout)
 //   warpgroups 1-2 : rows 0-63 / 64-127 of the tile: 4 x wgmma (K = 32 bytes each) per k-block
 //                 into a register accumulator; a stage is handed back once the wgmmas that read it
 //                 have completed (one arrival per warp)
-//   epilogue   : the accumulators are parked in a row-major shared-memory tile (over the drained
-//                 ring), then every warp stores 32 x 32 blocks: + bias (+ residual) (ReLU), to
-//                 interior rows only (the halo stays zero)
+//   epilogue   : from the accumulator registers, + bias (+ residual) (ReLU) and the rounding into
+//                 the staging tile, then one bulk store per interior row segment
+//                 (conv_epilogue.cuh); the halo border rows are never written
 // Roofline: tensor pipe (TF32 / FP16); algorithmic flops = 2 * rows_interior * taps*cin * cout.
 #include "host_util.h"
 #include "pdl.cuh"
@@ -74,17 +75,30 @@ __device__ __forceinline__ float rna_tf32(float x) {
 
 constexpr int kConvThreads = 384;  // producer warpgroup + two MMA / epilogue warpgroups
 
+// Shared memory: the whole 227 KB a CTA may use.  [0, RING_BYTES) is the stage ring; the mbarriers sit at the top;
+// the epilogue's staging tile [128][BN + 8] (output element type) ends where they begin, so it overlaps only the
+// last stages of the ring, or none.  A prefetched residual (which fills the staging tile) therefore waits only
+// for those stages to drain, and for layers with fewer k-blocks than free stages it waits for nothing.
 template <int BN, int STAGES>
 struct SmemLayout {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  // accumulator tile [128][BN + 8] fp32: the pad makes the fragment stores (8-byte pieces of 4 rows per
-  // half-warp) conflict-free; it reuses the ring, which is drained when the tile is written
+  static constexpr int TOTAL = 232448 - 1024;  // less the slack for the manual 1024-byte alignment
+  static constexpr int BAR_OFF = TOTAL - 256;  // full[STAGES], empty[STAGES], residual, drain
+  static_assert(RING_BYTES <= BAR_OFF && (2 * STAGES + 2) * 8 <= 256, "stage ring and barriers exceed 227 KB");
+  // split-K: fp32 partial tile [128][BN + 8] parked over the drained ring; the pad makes the fragment stores
+  // (8-byte pieces of 4 rows per half-warp) conflict-free
   static constexpr int ACC_STRIDE = BN + 8;
-  static constexpr int ACC_BYTES = BM * ACC_STRIDE * 4;
-  static constexpr int BAR_OFF = ((RING_BYTES > ACC_BYTES ? RING_BYTES : ACC_BYTES) + 7) & ~7;
-  static constexpr int TOTAL = BAR_OFF + 2 * STAGES * 8;
+  static_assert(BM * ACC_STRIDE * 4 <= BAR_OFF, "split-K partial tile exceeds the ring");
+  __host__ __device__ static constexpr int stage_off(int esz) {
+    return (BAR_OFF - BM * kStageStride<BN> * esz) & ~127;
+  }
+  // ring stages below the staging tile
+  __host__ __device__ static constexpr int free_stages(int esz) {
+    return stage_off(esz) / STAGE_BYTES < STAGES ? stage_off(esz) / STAGE_BYTES : STAGES;
+  }
+  static_assert(free_stages(4) >= 1, "the fp32 staging tile leaves no ring stage free");
 };
 
 template <int BN, int STAGES, bool F16>
@@ -98,6 +112,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* res_bar = empty_bar + STAGES;
+  uint64_t* drain_bar = res_bar + 1;  // the ring stages under the staging tile are released for the last time
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
@@ -109,6 +125,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int S = p.splits;
   const int j0 = static_cast<int>(static_cast<int64_t>(split) * iters / S);
   const int j1 = static_cast<int>(static_cast<int64_t>(split + 1) * iters / S);
+  const int esz = p.f16_out ? 2 : 4;
+  uint8_t* stile = smem + L::stage_off(esz);
+  // With a residual (applied here unless split-K's second pass does it), k-block `it` uses stage (it + rot) % STAGES:
+  // the rotation puts the last k-blocks on the free stages, so the residual may fill the staging tile while they run.
+  // A stage's n-th use is still k-block it / STAGES == n of it, so the barrier parities are unchanged.
+  const bool res_here = p.residual && S == 1;
+  const int nfree = res_here ? L::free_stages(esz) : STAGES;
+  const int rot = res_here ? ((nfree - (j1 - j0)) % STAGES + STAGES) % STAGES : 0;
+  // k-blocks before drain_it use stages under the staging tile; when k-block drain_it's wgmmas are issued and the
+  // previous ones completed, those stages are free for good (a stage's empty barrier cycles too fast for a later
+  // parity wait to tell its phases apart)
+  const int drain_it = res_here ? (j1 - j0) - nfree : 0;
 
   if (threadIdx.x == 0) {
     sm90::prefetch_tmap(&tmA);
@@ -117,6 +145,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       sm90::mbar_init(&full_bar[s], 1);
       sm90::mbar_init(&empty_bar[s], 8);  // one arrival per MMA warp
     }
+    sm90::mbar_init(res_bar, 1);
+    sm90::mbar_init(drain_bar, 8);  // one arrival per MMA warp
     sm90::fence_barrier_init();
   }
   __syncthreads();
@@ -126,10 +156,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (warp < 4) {
     sm90::setmaxnreg_dec<40>();
+    if (warp == 1 && res_here) {
+      // residual prefetch: once no k-block uses the ring stages under the staging tile any more, bulk-load the rows
+      if (drain_it > 0) sm90::mbar_wait_backoff(drain_bar, 0, p.err, 103, 64);
+      conv_prefetch_residual<BN>(stile, res_bar, lane, m0, n0, p);
+    }
     if (threadIdx.x == 0) {
       const int wp = p.w + 2;
       for (int j = j0, it = 0; j < j1; ++j, ++it) {
-        const int s = it % STAGES;
+        const int s = (it + rot) % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         const int t = j / p.kblocks;
         const int kb = j - t * p.kblocks;
@@ -154,7 +189,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   int prev = -1;
   for (int j = j0, it = 0; j < j1; ++j, ++it) {
-    const int s = it % STAGES;
+    const int s = (it + rot) % STAGES;
     sm90::mbar_wait(&full_bar[s], (it / STAGES) & 1, p.err, 102);
     const uint32_t sa = sm90::smem_u32(smem + s * L::STAGE_BYTES);
     const uint64_t da = sm90::make_desc_sw128(sa + wg * 64 * 128);
@@ -165,15 +200,22 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int k = 0; k < 4; ++k) sm90::wgmma<BN, F16>(acc, da + 2 * k, db + 2 * k, (j != j0 || k != 0) ? 1u : 0u);
     sm90::wgmma_commit();
     sm90::wgmma_wait<1>();  // the previous k-block's wgmmas are done: its stage may be refilled
-    if (prev >= 0 && lane == 0) sm90::mbar_arrive(&empty_bar[prev]);
+    if (prev >= 0 && lane == 0) {
+      sm90::mbar_arrive(&empty_bar[prev]);
+      if (it == drain_it) sm90::mbar_arrive(drain_bar);
+    }
     prev = s;
   }
   sm90::wgmma_wait<0>();
   sm90::fence_acc(acc);
 
   // both warpgroups have finished reading the ring (and every TMA write into it was waited for): the
-  // accumulator tile may overwrite it
+  // staging / partial tile may overwrite it
   sm90::named_sync(1, 256);
+  if (S == 1) {
+    conv_epilogue_tile<BN>(acc, stile, res_bar, wg, tw, m0, n0, p);
+    return;
+  }
   float* tile = reinterpret_cast<float*>(smem);
   {
     const int r = wg * 64 + (tw >> 5) * 16 + ((tw & 31) >> 2);
@@ -186,37 +228,21 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
   sm90::named_sync(1, 256);
 
-  // epilogue: 32-row x 32-column blocks, consumer warp cw takes blocks cw, cw + 8, ...
+  // split-K: park the fp32 partial tile in the workspace [tile][split][128 rows][BN] in 32-row x 32-column blocks,
+  // consumer warp cw takes blocks cw, cw + 8, ...; splitk_epilogue_kernel (next launch) sums the S partials in split
+  // order and applies bias / residual / ReLU / conversion
   const int cw = warp - 4;
-  const int wp = p.w + 2;
-  const int64_t per_img = static_cast<int64_t>(p.h + 2) * wp;
 #pragma unroll 1
   for (int blk = cw; blk < 4 * (BN / 32); blk += 8) {
     const int rb = blk & 3, cb = blk >> 2;
-    const int64_t row0 = m0 + rb * 32;
     const float* src = tile + rb * 32 * L::ACC_STRIDE + cb * 32;
-    if (S > 1) {
-      // split-K: park the fp32 partial block in the workspace [tile][split][128 rows][BN]; splitk_epilogue_kernel
-      // (next launch) sums the S partials in split order and applies bias / residual / ReLU / conversion
-      float* dst = p.sk_ws + (((static_cast<int64_t>(nt) * m_tiles + mt) * S + split) * BM + rb * 32) * BN + cb * 32;
-      const int c4 = lane & 7, rsub = lane >> 3;
+    float* dst = p.sk_ws + (((static_cast<int64_t>(nt) * m_tiles + mt) * S + split) * BM + rb * 32) * BN + cb * 32;
+    const int c4 = lane & 7, rsub = lane >> 3;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int rr = i * 4 + rsub;
-        *reinterpret_cast<float4*>(dst + rr * BN + c4 * 4) = *reinterpret_cast<const float4*>(src + rr * L::ACC_STRIDE + c4 * 4);
-      }
-      continue;
+    for (int i = 0; i < 8; ++i) {
+      const int rr = i * 4 + rsub;
+      *reinterpret_cast<float4*>(dst + rr * BN + c4 * 4) = *reinterpret_cast<const float4*>(src + rr * L::ACC_STRIDE + c4 * 4);
     }
-    const int64_t r = row0 + lane;
-    bool interior = false;
-    if (r < p.rows) {
-      const int64_t rem = r % per_img;
-      const int y = static_cast<int>(rem / wp);
-      const int x = static_cast<int>(rem - static_cast<int64_t>(y) * wp);
-      interior = (y >= 1) && (y <= p.h) && (x >= 1) && (x <= p.w);
-    }
-    const uint32_t interior_mask = __ballot_sync(0xffffffffu, interior);
-    conv_epilogue_block(src, L::ACC_STRIDE, lane, row0, interior_mask, n0 + cb * 32, p);
   }
 }
 
@@ -276,7 +302,7 @@ template <int BN, int STAGES, bool F16>
 int launch(const mivos_conv_args* a, const ConvParams& p, cudaStream_t stream) {
   using L = SmemLayout<BN, STAGES>;
   constexpr int smem_bytes = L::TOTAL + 1024;  // slack for the manual 1024B alignment
-  static_assert(smem_bytes <= 232448, "stage ring exceeds the 227 KB a CTA may use");
+  static_assert(smem_bytes <= 232448, "shared memory exceeds the 227 KB a CTA may use");
   auto kernel = conv_gemm_kernel<BN, STAGES, F16>;
   static bool configured = false;
   if (!configured) {
@@ -421,7 +447,8 @@ extern "C" MIVOS_API int mivos_conv_gemm(const mivos_conv_args* a, mivos_stream_
   MIVOS_REQUIRE(!a->residual || (a->res_cstride % eo == 0 && a->res_coff % eo == 0), "conv_gemm: residual stride/offset must be multiples of %d", eo);
   MIVOS_REQUIRE(!a->out_relu || (a->out_relu_cstride % eo == 0 && a->out_relu_coff % eo == 0), "conv_gemm: out_relu stride/offset must be multiples of %d", eo);
   MIVOS_REQUIRE((reinterpret_cast<uintptr_t>(a->in) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->weight) & 15) == 0 &&
-                (reinterpret_cast<uintptr_t>(a->out) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->bias) & 15) == 0,
+                (reinterpret_cast<uintptr_t>(a->out) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->bias) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(a->residual) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->out_relu) & 15) == 0,
                 "conv_gemm: pointers must be 16-byte aligned");
   MIVOS_REQUIRE(a->n > 0 && a->h > 0 && a->w > 0, "conv_gemm: bad map dims");
 

@@ -103,6 +103,27 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// 1-D bulk copy global -> shared of `bytes` (a multiple of 16; both addresses 16-byte aligned), completing on `bar`
+// as transaction bytes.
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(gmem_src)), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
+// 1-D bulk copy shared -> global (same size / alignment rules), tracked in the issuing thread's bulk groups.
+__device__ __forceinline__ void bulk_store(void* gmem_dst, const void* smem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;\n" ::"l"(reinterpret_cast<uint64_t>(gmem_dst)),
+               "r"(smem_u32(smem_src)), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+// Waits until every committed bulk store of this thread has finished READING shared memory (its source may be
+// overwritten or freed); the global writes complete on their own.
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
+// Makes this thread's generic-proxy writes to shared memory visible to later async-proxy (bulk copy) reads.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+
 // ----------------------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor, K-major operand, SWIZZLE_128B: rows of 128 bytes, 8-row groups
 // 1024 bytes apart (SBO), written by a TMA box {128 bytes, rows} with CU_TENSOR_MAP_SWIZZLE_128B.

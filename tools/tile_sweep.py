@@ -62,7 +62,9 @@ for (n, h, w, cin, cout, ks, res) in SHAPES:
         row.append(f"{1e3 * e0.elapsed_time(e1) / (3 * REPS):6.1f}")
     lib.mivos_conv_tile_override(0, 0)
     fl = 2.0 * n * h * w * ks * ks * cin * cout
+    # least HBM traffic: the input map, the residual and the output once each (interior pixels), and the weights
+    hbm = (2 if DT == torch.float16 else 4) * (n * h * w * (cin + cout * (2 if res else 1)) + ks * ks * cin * cout)
     best = min(float(v) for v in row[1:] if v.strip() != "-")
-    print(f"n={n} {h:3d}x{w:3d} {cin:4d}->{cout:4d} k{ks} res={int(res)} | auto {row[0]} | 32:{row[1]} 64:{row[2]} 128:{row[3]} 256:{row[4]} | best {fl / best / 1e6:7.1f} TF/s")
+    print(f"n={n} {h:3d}x{w:3d} {cin:4d}->{cout:4d} k{ks} res={int(res)} | auto {row[0]} | 32:{row[1]} 64:{row[2]} 128:{row[3]} 256:{row[4]} | best {fl / best / 1e6:7.1f} TF/s {hbm / best / 1e3:7.1f} GB/s")
 _lib.poll_kernel_error()
 print("done")
