@@ -217,6 +217,22 @@ MIVOS_API int mivos_memory_read(const float* bank_k, const float* bank_v, int64_
                       void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
                       int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
                       int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
+/* Dense space-time memory read — EvalMemoryReader.forward with top_k=None (prop_net.py:99-102): for
+ * every query pixel q, softmax over ALL `slots` live bank slots of keys . qk / sqrt(128), then the
+ * value-weighted read-out (the full 2*(128+512)*slots*hw flops per object, on the tensor cores:
+ * 3xTF32 scores, online softmax, TF32 P.V, a second launch merging the chunks of the memory axis).
+ * Operands, query sets (q_div), output window (out_cstride / out_coff / out_halo_h,w, out_f16) and
+ * dyn_slots as for mivos_memory_read; 1 <= slots <= slots_cap.  Slots at or past the live count take
+ * no part (they may hold stale data or NaN).  The partition of the memory axis depends on hw alone,
+ * so eager (slots = n) and graph-sized (dyn_slots = n) reads, one q_div call and the per-set calls,
+ * and repeated calls give the same bits.  `workspace` sized by mivos_memory_read_dense_workspace()
+ * for the bank capacity (256-byte aligned); returns -1 on bad arguments.                         */
+MIVOS_API int64_t mivos_memory_read_dense_workspace(int k_objects, int64_t slots_cap, int hw);
+MIVOS_API int mivos_memory_read_dense(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int q_div,
+                      void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      void* workspace, int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
+                      mivos_stream_t stream);
 /* Diagnostic, synchronising: candidate statistics of the last tensor-core-path read in `workspace`:
  * out[0] total candidates, out[1] max per (object, query), out[2] queries served by the exact
  * fallback, out[3] splits of the memory axis.                                                    */

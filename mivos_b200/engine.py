@@ -200,7 +200,8 @@ class _ResNetTrunk:
 
 
 class PropagationEngine(_ResNetTrunk):
-    def __init__(self, state_dict: Dict[str, torch.Tensor], device, top_k: int, act_dtype: Optional[torch.dtype] = None):
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device, top_k: Optional[int],
+                 act_dtype: Optional[torch.dtype] = None):
         self.device = torch.device(device)
         self.top_k = top_k
         self.act_dtype = act_dtype or act_dtype_from_env()
@@ -354,6 +355,24 @@ class PropagationEngine(_ResNetTrunk):
                       round_tf32=out_relu_only)
         return out
 
+    @property
+    def min_live_slots(self) -> int:
+        """Fewest live bank slots a read accepts: top_k for the top-k read (as torch.topk), 1 for the dense read."""
+        return 1 if self.top_k is None else self.top_k
+
+    def _memory_read(self, bank_k, bank_v, slots: int, qk, n: int, cat, h16: int, w16: int, dyn_slots, q_div: int):
+        """The memory read of n objects into channels [0, 512) of `cat`: the top-k read (prop_net.py:47-73), or
+        the dense read of the reference's top_k=None (prop_net.py:99-102).  The only place that tells them apart."""
+        hw = h16 * w16
+        if self.top_k is None:
+            wsp = self.ws.raw("memread_dense", ops.memory_read_dense_workspace_bytes(n, bank_k.shape[1], hw))
+            ops.memory_read_dense(bank_k, bank_v, slots, qk, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
+                                  dyn_slots=dyn_slots, q_div=q_div)
+        else:
+            wsp = self.ws.raw("memread", ops.memory_read_workspace_bytes(n, slots, hw, self.top_k))
+            ops.memory_read(bank_k, bank_v, slots, qk, self.top_k, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
+                            algo=self.memread_algo, dyn_slots=dyn_slots, q_div=q_div)
+
     def segment(self, bank_k, bank_v, slots: int, qs: QueryState, K: int, *, want_raw=False, want_prob=True,
                 prob_out=None, dyn_slots=None):
         """segment_with_query (prop_net.py:170-181) + aggregate_wbg(keep_bg=True)
@@ -363,9 +382,7 @@ class PropagationEngine(_ResNetTrunk):
         h16, w16 = H // 16, W // 16
         hw = h16 * w16
         cat = ws.halo("cat", K, h16, w16, 1024)
-        wsp = ws.raw("memread", ops.memory_read_workspace_bytes(K, slots, hw, self.top_k))
-        ops.memory_read(bank_k, bank_v, slots, qs.qk, self.top_k, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
-                        algo=self.memread_algo, dyn_slots=dyn_slots)
+        self._memory_read(bank_k, bank_v, slots, qs.qk, K, cat, h16, w16, dyn_slots, 0)
         ops.halo_copy(qs.kv, cat, K, h16, w16, 512, src_coff=128, dst_coff=512)  # cat([readout, v16]) :178-179
         catr = ws.halo("catr", K, h16, w16, 1024)
         ops.halo_copy(cat, catr, K, h16, w16, 1024, relu=True)
@@ -409,9 +426,7 @@ class PropagationEngine(_ResNetTrunk):
         N = C * K
         cat = ws.halo("cat", N, h16, w16, 1024)
         # ONE read for the C clips: object c*K + k reads query set c (q_div = K objects per set)
-        wsp = ws.raw("memread", ops.memory_read_workspace_bytes(N, slots, hw, self.top_k))
-        ops.memory_read(bank_k, bank_v, slots, qb.qk, self.top_k, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
-                        algo=self.memread_algo, dyn_slots=dyn_slots, q_div=K)
+        self._memory_read(bank_k, bank_v, slots, qb.qk, N, cat, h16, w16, dyn_slots, K)
         ops.halo_copy(qb.kv, cat, N, h16, w16, 512, src_coff=128, dst_coff=512)  # clip c's v16 over its K objects
         catr = ws.halo("catr", N, h16, w16, 1024)
         ops.halo_copy(cat, catr, N, h16, w16, 1024, relu=True)

@@ -101,7 +101,7 @@ class _FrameStep:
         """`frame` [1,3,nh,nw] and `qs_cached` on the device; `prob_dst` [(K+1),T,1,nh,nw]: the step writes its result
         planes to prob_dst[:, ti] itself (None: the result is only left in self.prob, e.g. for fuse_one_frame)."""
         assert visible_frames <= self.cap_frames and m_front < self.cap_frames
-        if visible_frames * self.hw < self.net.top_k:  # same rule as the eager path (mivos_memory_read) and torch.topk
+        if visible_frames * self.hw < self.net.min_live_slots:  # same rule as the eager path (mivos_memory_read) and torch.topk
             raise _lib.MivosError(f"memory_read: {visible_frames * self.hw} live bank slots < top_k {self.net.top_k}")
         srcs = [frame.data_ptr() if memorize else 0, qs_cached.kv.data_ptr(), qs_cached.qk.data_ptr(),
                 qs_cached.s8.data_ptr(), qs_cached.s4.data_ptr()]

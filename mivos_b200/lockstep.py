@@ -98,7 +98,7 @@ class _LockStep:
         [(K+1),T,1,nh,nw]: the step writes clip c's result planes to prob_dsts[c][:, ti] itself (None: results are
         only left in self.prob[c])."""
         assert visible <= self.cap_frames and m_front < self.cap_frames
-        if visible * self.hw < self.net.top_k:  # same rule as the eager path (mivos_memory_read) and torch.topk
+        if visible * self.hw < self.net.min_live_slots:  # same rule as the eager path (mivos_memory_read) and torch.topk
             raise MivosError(f"memory_read: {visible * self.hw} live bank slots < top_k {self.net.top_k}")
         C, K = self.C, self.K
         if isinstance(cached, QueryState):  # the C clips' states of this frame, contiguous (joint query pass)

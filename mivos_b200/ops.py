@@ -368,6 +368,37 @@ def memory_read(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torc
     return (out, idx, val) if want_topk else out
 
 
+def memory_read_dense_workspace_bytes(k: int, slots_cap: int, hw: int) -> int:
+    """Workspace of memory_read_dense for k objects over a bank of `slots_cap` slots (the capacity, not the live count)."""
+    n = _lib.load().mivos_memory_read_dense_workspace(k, slots_cap, hw)
+    if n < 0:
+        raise _lib.MivosError(f"memory_read_dense_workspace: bad arguments (k={k} slots_cap={slots_cap} hw={hw})")
+    return int(n)
+
+
+def memory_read_dense(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, out: torch.Tensor, *,
+                      out_coff: int = 0, halo_hw=None, workspace: Optional[torch.Tensor] = None,
+                      dyn_slots: Optional[torch.Tensor] = None, q_div: int = 0):
+    """The reference's dense read (EvalMemoryReader with top_k=None): softmax over all `slots` live bank slots.
+    Operands, query sets (q_div), output window and dyn_slots as for memory_read."""
+    _req(bank_k), _req(bank_v), _req(qk), _req_act(out)
+    k, cap = bank_k.shape[0], bank_k.shape[1]
+    hw = qk.shape[-2]
+    if qk.dim() == 3 and (q_div < 1 or (k + q_div - 1) // q_div != qk.shape[0]):
+        raise _lib.MivosError(f"memory_read_dense: {qk.shape[0]} query sets for {k} objects need q_div = objects per set (got {q_div})")
+    if qk.dim() == 2 and q_div != 0:
+        raise _lib.MivosError("memory_read_dense: q_div needs a [sets,hw,128] query tensor")
+    need = memory_read_dense_workspace_bytes(k, cap, hw)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=qk.device)
+    hh, ww = halo_hw if halo_hw is not None else (0, 0)
+    check(_lib.lib().mivos_memory_read_dense(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, q_div, _ptr(out),
+                                             out.shape[-1], out_coff, hh, ww, _ptr(workspace), workspace.numel(),
+                                             _ptr(dyn_slots), _f16(out), _stream()),
+          "mivos_memory_read_dense")
+    return out
+
+
 def upsample4x_sigmoid_aggregate(logits: torch.Tensor, k: int, h4: int, w4: int, coff: int = 0,
                                  want_raw: bool = False, want_prob: bool = True,
                                  raw_out: Optional[torch.Tensor] = None, prob_out: Optional[torch.Tensor] = None,

@@ -29,8 +29,9 @@ class _Reader(nn.Module):
 
 
 class PropagationNetwork(nn.Module):
-    def __init__(self, top_k: int = 50, act_dtype: Optional[torch.dtype] = None):
-        """`act_dtype` (extension over the reference signature, prop_net.py:132): torch.float32 (TF32
+    def __init__(self, top_k: Optional[int] = 50, act_dtype: Optional[torch.dtype] = None):
+        """`top_k` None selects the reference's dense read (softmax over every bank slot, prop_net.py:99-102).
+        `act_dtype` (extension over the reference signature, prop_net.py:132): torch.float32 (TF32
         tensor-core path) or torch.float16; None reads MIVOS_ACT_DTYPE (engine.act_dtype_from_env)."""
         super().__init__()
         self.act_dtype = act_dtype
@@ -62,8 +63,13 @@ class PropagationNetwork(nn.Module):
         return super().load_state_dict(*a, **k)
 
     @property
-    def top_k(self) -> int:
+    def top_k(self) -> Optional[int]:
         return self.memory.top_k
+
+    @property
+    def min_live_slots(self) -> int:
+        """Fewest live bank slots the memory read accepts: top_k, or 1 for the dense read (top_k=None)."""
+        return 1 if self.memory.top_k is None else self.memory.top_k
 
     def engine(self) -> PropagationEngine:
         """The packed network for (device, top_k, activation type).  The activation type is the
