@@ -172,13 +172,13 @@ def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], bn=None, strid
                       cin, cin_pad, cout, cout_pad, taps, kh, stride)
 
 
-def conv_gemm(x: torch.Tensor, pc: PackedConv, n: int, h: int, w: int, out: torch.Tensor, *,
+def conv_args(x: torch.Tensor, pc: PackedConv, n: int, h: int, w: int, out: torch.Tensor, *,
               in_coff: int = 0, out_coff: int = 0, relu: bool = False,
               residual: Optional[torch.Tensor] = None, res_coff: int = 0,
               out_relu: Optional[torch.Tensor] = None, out_relu_coff: int = 0,
-              round_tf32: bool = False, splitk_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[HALO (n,h,w)] = conv(x) (+residual)(relu).  `x` is a HALO map of the same (n,h,w) for
-    taps=9 / 1x1, or a pre-gathered matrix whose rows are the HALO rows of the output map."""
+              round_tf32: bool = False, splitk_ws: Optional[torch.Tensor] = None) -> ConvArgs:
+    """The validated mivos_conv_args block of a conv_gemm call (the same arguments), without launching it.
+    The tensors must outlive any use of the returned block: it holds their raw device pointers."""
     _req_act(x), _req_act(out)
     if _f16(x) != _f16(pc.weight):
         raise _lib.MivosError("conv_gemm: input map and packed weights differ in element type")
@@ -214,6 +214,14 @@ def conv_gemm(x: torch.Tensor, pc: PackedConv, n: int, h: int, w: int, out: torc
     if splitk_ws is not None:  # zero-initialised scratch (split_k_workspace) owned by this stream's workspace
         a.splitk_ws = splitk_ws.data_ptr()
         a.splitk_ws_bytes = splitk_ws.numel() * splitk_ws.element_size()
+    return a
+
+
+def conv_gemm(x: torch.Tensor, pc: PackedConv, n: int, h: int, w: int, out: torch.Tensor, **kw) -> torch.Tensor:
+    """out[HALO (n,h,w)] = conv(x) (+residual)(relu).  `x` is a HALO map of the same (n,h,w) for
+    taps=9 / 1x1, or a pre-gathered matrix whose rows are the HALO rows of the output map.  Keywords as
+    conv_args: in_coff, out_coff, relu, residual, res_coff, out_relu, out_relu_coff, round_tf32, splitk_ws."""
+    a = conv_args(x, pc, n, h, w, out, **kw)
     check(_lib.lib().mivos_conv_gemm(C.byref(a), _stream()), "mivos_conv_gemm")
     return out
 

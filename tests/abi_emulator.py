@@ -52,10 +52,10 @@ def conv_gemm(x, pc, n, h, w, out, *, in_coff=0, out_coff=0, relu=False, residua
     if relu:
         v = v.clamp_min(0)
     o = out.reshape(-1, out.shape[-1])
-    o[:rows][inner, out_coff:out_coff + pc.cout] = v[inner]
+    o[:rows][inner, out_coff:out_coff + pc.cout] = v[inner].to(o.dtype)
     if out_relu is not None:
         r = out_relu.reshape(-1, out_relu.shape[-1])
-        r[:rows][inner, out_relu_coff:out_relu_coff + pc.cout] = v[inner].clamp_min(0)
+        r[:rows][inner, out_relu_coff:out_relu_coff + pc.cout] = v[inner].clamp_min(0).to(r.dtype)
     return out
 
 

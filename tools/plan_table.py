@@ -1,8 +1,8 @@
 """CPU-only: the tile width / split-K plan `mivos_conv_gemm` picks (mivos_conv_plan, pure host arithmetic)
 for every convolution of the sequential step (segment + memorize) at cfg-2, for a batch of n = C*K maps —
-n = 1 is one clip, n = 4 a lock-step lane of four.  Prints row tiles, CTAs, waves on 148 SMs and the
+n = 1 is one clip, n = 4 a lock-step lane of four.  Prints row tiles, CTAs, waves on the SMs and the
 tensor work per launch, to see which layers the batch lifts over one wave and which it does not.
-Usage: python tools/plan_table.py [n ...=1 4 8]"""
+Usage: python tools/plan_table.py [--sms S=132 (H100 SXM)] [n ...=1 4 8]"""
 import ctypes as C
 import os
 import sys
@@ -10,7 +10,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from mivos_b200 import _lib  # noqa: E402
 
-SMS = 148
+SMS = 132  # H100 SXM
 H, W = 480, 864
 
 
@@ -44,7 +44,7 @@ def layers():
     return out
 
 
-def plan(n, h, w, cin, cout, ks, residual):
+def plan(n, h, w, cin, cout, ks, residual, sms=SMS):
     a = _lib.ConvArgs()
     a.n, a.h, a.w = n, h, w
     a.cin_pad = (cin + 63) // 64 * 64
@@ -54,7 +54,7 @@ def plan(n, h, w, cin, cout, ks, residual):
     a.residual = 1 if residual else 0
     a.splitk_ws, a.splitk_ws_bytes = 1, 48 << 20
     bn, sp = C.c_int(0), C.c_int(0)
-    assert _lib.load().mivos_conv_plan(C.byref(a), SMS, C.byref(bn), C.byref(sp)) == 0
+    assert _lib.load().mivos_conv_plan(C.byref(a), sms, C.byref(bn), C.byref(sp)) == 0
     rows = n * (h + 2) * (w + 2)
     mt = (rows + 127) // 128
     ctas = mt * (a.cout_pad // bn.value) * sp.value
@@ -62,18 +62,21 @@ def plan(n, h, w, cin, cout, ks, residual):
 
 
 def main():
-    ns = [int(x) for x in sys.argv[1:]] or [1, 4, 8]
+    args, sms = sys.argv[1:], SMS
+    if args[:1] == ["--sms"]:
+        sms, args = int(args[1]), args[2:]
+    ns = [int(x) for x in args] or [1, 4, 8]
     print(f"{'layer':44s} {'x':>2s} " + " ".join(f"| n={n}: BN sp tiles CTAs waves  GF" for n in ns))
     tot = {n: 0.0 for n in ns}
     for name, h, w, cin, cout, ks, cnt, res in layers():
         cells = []
         for n in ns:
-            bn, sp, mt, ctas = plan(n, h, w, cin, cout, ks, res)
+            bn, sp, mt, ctas = plan(n, h, w, cin, cout, ks, res, sms)
             gf = 2.0 * n * h * w * cin * cout * (9 if ks == 3 else 1) / 1e9
-            cells.append(f"| {bn:8d} {sp:2d} {mt:5d} {ctas:4d} {ctas / SMS:5.2f} {gf:5.1f}")
-            tot[n] += ctas / SMS * cnt
+            cells.append(f"| {bn:8d} {sp:2d} {mt:5d} {ctas:4d} {ctas / sms:5.2f} {gf:5.1f}")
+            tot[n] += ctas / sms * cnt
         print(f"{name:44s} {cnt:2d} " + " ".join(cells))
-    print("sum of (CTAs/148) x count per frame-step: " + ", ".join(f"n={n}: {tot[n]:.1f} ({tot[n] / n:.1f} per clip)" for n in ns))
+    print(f"sum of (CTAs/{sms}) x count per frame-step: " + ", ".join(f"n={n}: {tot[n]:.1f} ({tot[n] / n:.1f} per clip)" for n in ns))
 
 
 if __name__ == "__main__":
