@@ -359,10 +359,6 @@ int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits
   // through L2 and a second (HBM-bound, PDL-chained) launch that sums them and applies the
   // epilogue, ~8 us = 700 KB-equivalents — it pays only for the K >= 9 x 512 layers of the
   // 1/16-resolution maps.  Needs the caller's workspace.
-  static const bool allow_splitk = [] {  // MIVOS_CONV_SPLITK=0: A/B measurements
-    const char* e = getenv("MIVOS_CONV_SPLITK");
-    return !(e && e[0] == '0');
-  }();
   int bn = 32, splits = 1;
   double best_cost = 1e300;
   const int iters_total = a->taps * kblocks;
@@ -371,7 +367,7 @@ int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits
     const int64_t tiles = mtiles * (a->cout_pad / cand);
     for (int sp = 1; sp <= 8; ++sp) {
       if (sp > 1) {
-        if (!allow_splitk || !a->splitk_ws || iters_total / sp < 4 || tiles * sp > 2 * sms || tiles > kSkCounterBytes / 4) break;
+        if (!a->splitk_ws || iters_total / sp < 4 || tiles * sp > 2 * sms || tiles > kSkCounterBytes / 4) break;
         if (kSkCounterBytes + tiles * sp * BM * cand * 4 > a->splitk_ws_bytes) break;
       }
       const double rounds = static_cast<double>((tiles * sp + sms - 1) / sms);

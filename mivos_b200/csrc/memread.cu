@@ -31,21 +31,14 @@ extern std::atomic<int64_t> g_launches;
 MemreadPlan memread_plan(int k_objects, int64_t slots, int hw, int top_k, int algo) {
   MemreadPlan pl;
   pl.algo = algo;
-  if (algo == MIVOS_MEMREAD_TCGEN05) {
-    pl.qtile = 128;
-    pl.slot_tile = 256;
-    pl.kcap = kTcCandCap;
-  } else {
-    pl.qtile = 32;
-    pl.slot_tile = 128;
-    pl.kcap = top_k;
-  }
-  pl.qtiles = ceil_div(hw, pl.qtile);
-  const int64_t tiles = ceil_div64(slots, pl.slot_tile);
+  const bool tc = algo == MIVOS_MEMREAD_TCGEN05;
+  pl.kcap = tc ? kTcCandCap : top_k;
+  pl.qtiles = ceil_div(hw, tc ? 128 : 32);                // queries per CTA
+  const int64_t tiles = ceil_div64(slots, tc ? 256 : 128);  // bank slots per inner tile
   // exact path: ~2 CTAs per SM; tensor-core path: ONE wave of CTAs (~200 KB smem = 1 CTA/SM);
   // every split owns at least 4 slot tiles
   const int64_t sms = num_sms();
-  int64_t want = algo == MIVOS_MEMREAD_TCGEN05 ? sms / (static_cast<int64_t>(pl.qtiles) * k_objects)
+  int64_t want = tc ? sms / (static_cast<int64_t>(pl.qtiles) * k_objects)
                                                : ceil_div64(2 * sms, static_cast<int64_t>(pl.qtiles) * k_objects);
   int64_t max_by_tiles = tiles / 4 > 0 ? tiles / 4 : 1;
   int64_t s = want < max_by_tiles ? want : max_by_tiles;
@@ -53,19 +46,15 @@ MemreadPlan memread_plan(int k_objects, int64_t slots, int hw, int top_k, int al
   if (s > kMaxSplits) s = kMaxSplits;
   pl.tiles_per_split = static_cast<int>(ceil_div64(tiles, s));
   pl.splits = static_cast<int>(ceil_div64(tiles, pl.tiles_per_split));
-  pl.nlists = algo == MIVOS_MEMREAD_TCGEN05 ? pl.splits * kTcHalves : pl.splits;
+  pl.nlists = tc ? pl.splits * kTcHalves : pl.splits;
   const int64_t lists = static_cast<int64_t>(k_objects) * hw * pl.nlists;
-  pl.off_list = 0;
-  pl.off_cnt = lists * pl.kcap * 8 + (algo == MIVOS_MEMREAD_TCGEN05 ? 4096 : 0);  // plan_lists() aligns the lists to 4 KB
-  pl.off_flag = 0;  // (overflow flags live in the tail of the workspace: memread_tc_run)
+  pl.off_cnt = lists * pl.kcap * 8 + (tc ? 4096 : 0);  // plan_lists() aligns the lists to 4 KB
   pl.bytes = pl.off_cnt + lists * 4;
   pl.bytes = (pl.bytes + 255) & ~255ll;
   return pl;
 }
 
 namespace {
-
-constexpr float kSqrtCK = 11.313708498984761f;  // sqrt(128) rounded to fp32, as the reference's divisor
 
 constexpr int A1_THREADS = 256;
 constexpr int A1_Q = 32;
@@ -121,8 +110,8 @@ memread_exact_kernel(const float* __restrict__ bank_k, int64_t slots_cap, int64_
   }
   __syncthreads();
 
+  slots = live_slots(dyn_slots, slots, slots_cap);
   if (dyn_slots) {  // device-side slot count (CUDA-graph replay): fixed grid, ranges derived here
-    slots = *dyn_slots;
     const int tiles = static_cast<int>((slots + A1_S - 1) / A1_S);
     tiles_per_split = (tiles + splits - 1) / splits;
   }
@@ -260,20 +249,18 @@ __device__ __forceinline__ float warp_max_f(float v) {
 }
 
 __global__ void __launch_bounds__(B_THREADS)
-memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict__ bank_v,
-                      int64_t slots_cap, const float* __restrict__ qk, int hw, int q_div, int top_k,
-                      const SelectLists prim, const int prim_rescore, const SelectLists fb,
+memread_select_kernel(const MemreadArgs a, const int top_k, const SelectLists L, const int rescore,
                       int* __restrict__ flags, const int pass, const float* __restrict__ qnorm,
-                      const float* __restrict__ kmax2, const int* __restrict__ tau_g, void* __restrict__ out, int out_cstride,
-                      int out_coff, int halo_h, int halo_w, int out_f16, int* __restrict__ topk_idx,
-                      float* __restrict__ topk_val, int* err, const int n_queries) {
+                      const float* __restrict__ kmax2, const int* __restrict__ tau_g, int* __restrict__ topk_idx,
+                      float* __restrict__ topk_val, int* err) {
   mivos::pdl_prologue();
   extern __shared__ __align__(16) uint8_t sel_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t lq = static_cast<int64_t>(blockIdx.x) * kSelWarps + warp;  // = obj * hw + q
-  if (lq >= n_queries) return;
+  const int hw = a.hw;
+  if (lq >= static_cast<int64_t>(a.k_objects) * hw) return;
   const int obj = static_cast<int>(lq / hw), q = static_cast<int>(lq - static_cast<int64_t>(obj) * hw);
-  const int qset = q_div > 0 ? obj / q_div : 0;  // query set of this object (lock-step clips: one per clip)
+  const int qset = a.q_div > 0 ? obj / a.q_div : 0;  // query set of this object (lock-step clips: one per clip)
   uint8_t* wb = sel_smem + warp * ((kSelBytesPerWarp + 15) & ~15);
   float* cs = reinterpret_cast<float*>(wb);          // [B_MAXSURV] candidate scores
   int* ci = reinterpret_cast<int*>(cs + B_MAXSURV);  // [B_MAXSURV] candidate slots
@@ -285,13 +272,9 @@ memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict_
   int* offs = order + MAXK;                          // [kMaxLists + 1]
 
   // two-pass protocol (launch_select): pass 0 leaves the flagged queries to pass 1 and may flag more of them below;
-  // pass 1 serves the flagged queries only.  Each pass reads ITS lists (`prim`); `fb` is kept for callers that
-  // serve both kinds in one launch (none today).
+  // pass 1 serves the flagged queries only.  Each pass reads its own lists.
   const bool flagged = flags != nullptr && flags[lq] != 0;
   if (flags != nullptr && (pass == 0) == flagged) return;
-  const bool use_fb = false;
-  const SelectLists& L = use_fb ? fb : prim;
-  const int rescore = prim_rescore;
 
   // ---- list lengths -> exclusive prefix (the count loads of the lanes are independent)
   {
@@ -306,7 +289,7 @@ memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict_
     if (lane == L.splits - 1) offs[L.splits] = incl;
   }
   {
-    const float4 v = reinterpret_cast<const float4*>(qk + (static_cast<int64_t>(qset) * hw + q) * 128)[lane];
+    const float4 v = reinterpret_cast<const float4*>(a.qk + (static_cast<int64_t>(qset) * hw + q) * 128)[lane];
     float4 sq;
     sq.x = v.x / kSqrtCK; sq.y = v.y / kSqrtCK; sq.z = v.z / kSqrtCK; sq.w = v.w / kSqrtCK;
     reinterpret_cast<float4*>(qs)[lane] = sq;
@@ -320,10 +303,7 @@ memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict_
   // chunk might not fit; the rest is filtered from global memory below.
   const float margin = rescore ? kTcMarginFactor * qnorm[static_cast<int64_t>(qset) * hw + q] * sqrtf(kmax2[obj]) : 0.f;
   float cut0 = -INFINITY;
-  if (rescore && tau_g) {
-    const int o = tau_g[lq];
-    cut0 = __int_as_float(o >= 0 ? o : o ^ 0x7fffffff) - margin;
-  }
+  if (rescore && tau_g) cut0 = ordered_float(tau_g[lq]) - margin;
   int n = 0;       // staged candidates
   int i_next = 0;  // first candidate not looked at yet
   {
@@ -438,7 +418,7 @@ memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict_
     }
     n = m;
     // exact fp32 scores, one survivor per lane per pass (normally two passes: n ~ 2k + margin hits)
-    const float* keys = bank_k + static_cast<int64_t>(obj) * slots_cap * 128;
+    const float* keys = a.bank_k + static_cast<int64_t>(obj) * a.slots_cap * 128;
     for (int i = lane; i < n; i += 32) cs[i] = exact_score(keys + static_cast<int64_t>(ci[i]) * 128, qs);
     __syncwarp();
   } else if (n_all > i_next) {  // cannot happen: exact lists hold top_k entries per split
@@ -479,7 +459,7 @@ memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict_
   float4 acc[4];
 #pragma unroll
   for (int u = 0; u < 4; ++u) acc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-  const float4* vals = reinterpret_cast<const float4*>(bank_v + static_cast<int64_t>(obj) * slots_cap * 512);
+  const float4* vals = reinterpret_cast<const float4*>(a.bank_v + static_cast<int64_t>(obj) * a.slots_cap * 512);
   // rows in batches of 4 (16 independent 16-byte loads per lane in flight); the accumulation order per channel
   // stays ascending slot index
   for (int j0 = 0; j0 < kk; j0 += 4) {
@@ -507,33 +487,13 @@ memread_select_kernel(const float* __restrict__ bank_k, const float* __restrict_
       }
     }
   }
-  int64_t row;
-  if (halo_w > 0) {
-    const int y = q / halo_w, x = q - y * halo_w;
-    row = (static_cast<int64_t>(obj) * (halo_h + 2) + y + 1) * (halo_w + 2) + x + 1;
-  } else {
-    row = lq;
-  }
-#pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const int c = (lane + 32 * u) * 4;
-    if (out_f16) {
-      const __half2 h01 = __floats2half2_rn(acc[u].x, acc[u].y), h23 = __floats2half2_rn(acc[u].z, acc[u].w);
-      uint2 pk;
-      pk.x = *reinterpret_cast<const uint32_t*>(&h01);
-      pk.y = *reinterpret_cast<const uint32_t*>(&h23);
-      *reinterpret_cast<uint2*>(static_cast<__half*>(out) + row * out_cstride + out_coff + c) = pk;
-    } else {
-      *reinterpret_cast<float4*>(static_cast<float*>(out) + row * out_cstride + out_coff + c) = acc[u];
-    }
-  }
+  store_read_row(a, obj, q, lane, acc);
 }
 
 }  // namespace
 
-int launch_exact_candidates(const float* bank_k, int64_t slots_cap, int k_objects, int64_t slots,
-                            const float* qk, int hw, int q_div, int top_k, const MemreadPlan& pl, void* ws,
-                            const int* flags, const int* dyn_slots, cudaStream_t stream) {
+int launch_exact_candidates(const MemreadArgs& a, int top_k, const MemreadPlan& pl, void* ws, const int* flags,
+                            cudaStream_t stream) {
   static bool configured = false;
   if (!configured) {
     MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -541,65 +501,72 @@ int launch_exact_candidates(const float* bank_k, int64_t slots_cap, int k_object
     configured = true;
   }
   uint8_t* w = static_cast<uint8_t*>(ws);
-  dim3 grid(pl.qtiles, pl.splits, k_objects);
-  launch_pdl(memread_exact_kernel, grid, A1_THREADS, sizeof(A1Smem), stream, 
-      bank_k, slots_cap, slots, qk, hw, q_div, top_k, pl.tiles_per_split, pl.splits,
-      reinterpret_cast<int2*>(plan_lists(w, pl)),
-      reinterpret_cast<int*>(w + pl.off_cnt), flags, dyn_slots);
+  dim3 grid(pl.qtiles, pl.splits, a.k_objects);
+  launch_pdl(memread_exact_kernel, grid, A1_THREADS, sizeof(A1Smem), stream, a.bank_k, a.slots_cap, a.slots, a.qk, a.hw,
+             a.q_div, top_k, pl.tiles_per_split, pl.splits, reinterpret_cast<int2*>(plan_lists(w, pl)),
+             reinterpret_cast<int*>(w + pl.off_cnt), flags, a.dyn_slots);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
 }
 
-int launch_select(const float* bank_k, const float* bank_v, int64_t slots_cap, int k_objects,
-                  const float* qk, int hw, int q_div, int top_k, const MemreadPlan& pl, void* ws,
-                  const MemreadPlan* fbp, void* fb_ws, int* flags, int pass, const float* qnorm,
-                  const float* kmax2, const int* tau_g, void* out, int out_cstride, int out_coff, int halo_h,
-                  int halo_w, int out_f16, int32_t* topk_idx, float* topk_val, cudaStream_t stream) {
+int launch_select(const MemreadArgs& a, int top_k, const MemreadPlan& pl, void* ws, int* flags, int pass,
+                  const float* qnorm, const float* kmax2, const int* tau_g, int32_t* topk_idx, float* topk_val,
+                  cudaStream_t stream) {
   uint8_t* w = static_cast<uint8_t*>(ws);
-  SelectLists prim{reinterpret_cast<const int2*>(plan_lists(w, pl)), reinterpret_cast<const int*>(w + pl.off_cnt),
-                   pl.nlists, pl.kcap};
-  SelectLists fb = prim;
-  if (fbp) {
-    uint8_t* f = static_cast<uint8_t*>(fb_ws);
-    fb = SelectLists{reinterpret_cast<const int2*>(plan_lists(f, *fbp)), reinterpret_cast<const int*>(f + fbp->off_cnt),
-                     fbp->nlists, fbp->kcap};
-  }
+  const SelectLists lists{reinterpret_cast<const int2*>(plan_lists(w, pl)), reinterpret_cast<const int*>(w + pl.off_cnt),
+                          pl.nlists, pl.kcap};
   const int rescore = pl.algo == MIVOS_MEMREAD_TCGEN05 ? 1 : 0;
-  MIVOS_REQUIRE(prim.splits <= 32 && fb.splits <= 32, "memory_read: more than 32 candidate lists per query");
+  MIVOS_REQUIRE(lists.splits <= 32, "memory_read: more than 32 candidate lists per query");
   constexpr int smem = kSelWarps * ((kSelBytesPerWarp + 15) & ~15);
   static bool configured = false;
   if (!configured) {
     MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  const int n_queries = k_objects * hw;
-  dim3 grid(ceil_div(n_queries, kSelWarps));
-  launch_pdl(memread_select_kernel, grid, B_THREADS, smem, stream, bank_k, bank_v, slots_cap, qk, hw, q_div, top_k, prim, rescore, fb,
-                                                           flags, pass, qnorm, kmax2, tau_g, out, out_cstride,
-                                                           out_coff, halo_h, halo_w, out_f16, topk_idx, topk_val,
-                                                           device_error_flag(), n_queries);
+  dim3 grid(ceil_div(a.k_objects * a.hw, kSelWarps));
+  launch_pdl(memread_select_kernel, grid, B_THREADS, smem, stream, a, top_k, lists, rescore, flags, pass, qnorm, kmax2,
+             tau_g, topk_idx, topk_val, device_error_flag());
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
+}
+
+int memread_check_args(const MemreadArgs& a, const char* who) {
+  MIVOS_REQUIRE(a.bank_k && a.bank_v && a.qk && a.out, "%s: null pointer", who);
+  MIVOS_REQUIRE(a.k_objects >= 1 && a.k_objects <= kMaxObjects && a.hw >= 1, "%s: bad object/query count", who);
+  MIVOS_REQUIRE(a.q_div >= 0, "%s: q_div must be >= 0 (0: all objects read one query set)", who);
+  MIVOS_REQUIRE(a.out_cstride % 4 == 0 && a.out_coff % 4 == 0 && a.out_coff >= 0 && a.out_coff + 512 <= a.out_cstride,
+                "%s: output channel window does not fit", who);
+  MIVOS_REQUIRE(a.halo_w == 0 || (a.halo_w > 0 && a.halo_h * a.halo_w == a.hw), "%s: halo dims do not match hw", who);
+  MIVOS_REQUIRE(((reinterpret_cast<uintptr_t>(a.bank_k) | reinterpret_cast<uintptr_t>(a.bank_v) |
+                  reinterpret_cast<uintptr_t>(a.qk) | reinterpret_cast<uintptr_t>(a.out)) & 15) == 0,
+                "%s: bank, query and output pointers must be 16-byte aligned", who);
+  return MIVOS_OK;
+}
+
+MemreadWorkspace memread_workspace(int k_objects, int64_t slots, int hw, int top_k) {
+  MemreadWorkspace w;
+  w.tc = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_TCGEN05);
+  w.ex = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
+  const int64_t nq = static_cast<int64_t>(k_objects) * hw, nq64 = (nq + 63) & ~63ll;
+  w.off_ex = w.tc.bytes;
+  w.off_overflow = w.off_ex + w.ex.bytes;
+  w.off_kmax2 = w.off_overflow + nq64 * 4;
+  w.off_qs = w.off_kmax2 + kMaxObjects * 4;
+  w.off_qnorm = w.off_qs + nq * 128 * 4;
+  w.off_tau = w.off_qnorm + nq64 * 4;
+  w.bytes = w.off_tau + nq64 * 4 + 1024;
+  return w;
 }
 
 }  // namespace mivos
 
 using namespace mivos;
 
-// tail of the workspace after the two plans' lists: flags [K*hw] | key-norm maxima [kMaxObjects] | scaled queries
-// [K*hw*128] (one set per object at most) | their norms [K*hw, padded to 64] | shared thresholds [K*hw]
-static int64_t memread_tail_bytes(int k_objects, int hw) {
-  const int64_t nq = static_cast<int64_t>(k_objects) * hw, nq64 = (nq + 63) & ~63ll;
-  return (nq64 + kMaxObjects + nq * 128 + nq64 + nq64) * 4 + 1024;
-}
-
 extern "C" MIVOS_API int64_t mivos_memory_read_workspace(int k_objects, int64_t slots, int hw, int top_k) {
   if (k_objects < 1 || k_objects > kMaxObjects || slots < 1 || hw < 1 || top_k < 1 || top_k > MAXK) return -1;
-  const MemreadPlan a = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
-  const MemreadPlan b = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_TCGEN05);
-  return b.bytes + a.bytes + memread_tail_bytes(k_objects, hw);
+  return memread_workspace(k_objects, slots, hw, top_k).bytes;
 }
 
 extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* bank_v, int64_t slots_cap,
@@ -609,34 +576,26 @@ extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* ban
                                            float* topk_val, void* workspace, int64_t workspace_bytes,
                                            int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  MIVOS_REQUIRE(bank_k && bank_v && qk && out && workspace, "memory_read: null pointer");
+  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
+                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16};
+  const int rc = memread_check_args(a, "memory_read");
+  if (rc != MIVOS_OK) return rc;
   MIVOS_REQUIRE(top_k >= 1 && top_k <= MAXK, "memory_read: top_k %d outside [1,%d]", top_k, MAXK);
   MIVOS_REQUIRE(slots >= top_k && slots <= slots_cap && slots < (1ll << 31) - 65536,
                 "memory_read: bad slot count %lld (cap %lld, k %d)", (long long)slots, (long long)slots_cap, top_k);
-  MIVOS_REQUIRE(k_objects >= 1 && k_objects <= kMaxObjects && hw >= 1, "memory_read: bad object/query count");
-  MIVOS_REQUIRE(q_div >= 0, "memory_read: q_div must be >= 0 (0: all objects read one query set)");
-  MIVOS_REQUIRE(out_cstride % 4 == 0 && out_coff % 4 == 0 && out_coff + 512 <= out_cstride,
-                "memory_read: output channel window does not fit");
-  MIVOS_REQUIRE(out_halo_w == 0 || out_halo_h * out_halo_w == hw, "memory_read: halo dims do not match hw");
-  MIVOS_REQUIRE((reinterpret_cast<uintptr_t>(bank_k) & 15) == 0 && (reinterpret_cast<uintptr_t>(bank_v) & 15) == 0 &&
-                    (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
-                "memory_read: pointers must be 16-byte aligned (workspace 256)");
+  MIVOS_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
+                "memory_read: workspace null or not 256-byte aligned");
   const int64_t need = mivos_memory_read_workspace(k_objects, slots, hw, top_k);
   MIVOS_REQUIRE(workspace_bytes >= need, "memory_read: workspace %lld < %lld bytes", (long long)workspace_bytes, (long long)need);
-  if (algo == MIVOS_MEMREAD_AUTO) algo = memread_tc_available() ? MIVOS_MEMREAD_TCGEN05 : MIVOS_MEMREAD_EXACT_SIMT;
 
   if (algo == MIVOS_MEMREAD_EXACT_SIMT) {
     const MemreadPlan pl = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
-    int rc = launch_exact_candidates(bank_k, slots_cap, k_objects, slots, qk, hw, q_div, top_k, pl, workspace, nullptr, dyn_slots, stream);
-    if (rc != MIVOS_OK) return rc;
-    return launch_select(bank_k, bank_v, slots_cap, k_objects, qk, hw, q_div, top_k, pl, workspace, nullptr, nullptr,
-                         nullptr, 0, nullptr, nullptr, nullptr, out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, topk_idx,
-                         topk_val, stream);
+    const int rc_a = launch_exact_candidates(a, top_k, pl, workspace, nullptr, stream);
+    if (rc_a != MIVOS_OK) return rc_a;
+    return launch_select(a, top_k, pl, workspace, nullptr, 0, nullptr, nullptr, nullptr, topk_idx, topk_val, stream);
   }
-  if (algo == MIVOS_MEMREAD_TCGEN05) {
-    return memread_tc_run(bank_k, bank_v, slots_cap, k_objects, slots, qk, hw, q_div, top_k, out, out_cstride,
-                          out_coff, out_halo_h, out_halo_w, out_f16, topk_idx, topk_val, workspace, dyn_slots, stream);
-  }
+  if (algo == MIVOS_MEMREAD_AUTO || algo == MIVOS_MEMREAD_TCGEN05)
+    return memread_tc_run(a, top_k, topk_idx, topk_val, workspace, stream);
   set_last_error("memory_read: unknown algo %d", algo);
   return MIVOS_ERR_INVALID;
 }
@@ -647,14 +606,14 @@ extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* ban
 extern "C" MIVOS_API int mivos_memory_read_stats(const void* workspace, int k_objects, int64_t slots, int hw,
                                                  int top_k, int64_t* out) {
   MIVOS_REQUIRE(workspace && out, "memory_read_stats: null pointer");
-  const MemreadPlan tc = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_TCGEN05);
-  const MemreadPlan ex = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
+  const MemreadWorkspace ws = memread_workspace(k_objects, slots, hw, top_k);
+  const MemreadPlan& tc = ws.tc;
   const int64_t nq = static_cast<int64_t>(k_objects) * hw;
   int* cnt = new int[nq * tc.nlists];
   int* flg = new int[nq];
   const uint8_t* w = static_cast<const uint8_t*>(workspace);
   cudaError_t e1 = cudaMemcpy(cnt, w + tc.off_cnt, nq * tc.nlists * 4, cudaMemcpyDeviceToHost);
-  cudaError_t e2 = cudaMemcpy(flg, w + tc.bytes + ex.bytes, nq * 4, cudaMemcpyDeviceToHost);
+  cudaError_t e2 = cudaMemcpy(flg, w + ws.off_overflow, nq * 4, cudaMemcpyDeviceToHost);
   int64_t total = 0, mx = 0, flagged = 0;
   if (e1 == cudaSuccess && e2 == cudaSuccess) {
     for (int64_t q = 0; q < nq; ++q) {

@@ -1,7 +1,9 @@
-// Internal interface between the memory-read translation units (memread.cu, memread_tc.cu).
+// Internal interface between the memory-read translation units (memread.cu, memread_tc.cu, memread_dense.cu):
+// the operands of a read, the workspace layout of the top-k read, and the device pieces the kernels share.
 #pragma once
 #include "host_util.h"
 
+#include <cuda_fp16.h>
 #include <cstdint>
 
 namespace mivos {
@@ -19,18 +21,39 @@ constexpr int kTcHalves = 2;      // column halves of a slot tile, one thread (a
 constexpr int kMaxLists = kMaxSplits * kTcHalves;  // candidate lists per (object, query)
 // margin = 2*eps, eps = 1.05 * 2^-9 * ||q/sqrt(128)|| * max||key||  (see memread_tc.cu)
 constexpr float kTcMarginFactor = 2.0f * 1.05f * 0.001953125f;
+constexpr float kSqrtCK = 11.313708498984761f;  // sqrt(128) rounded to fp32, as the reference's divisor
+
+// Operands of one read (top-k or dense), as the C entry points receive them.
+struct MemreadArgs {
+  // bank: keys [k_objects, slots_cap, 128], values [k_objects, slots_cap, 512]; the first `slots` rows are live, or
+  // *dyn_slots of them when that optional device scalar is given (CUDA-graph replay)
+  const float* bank_k;
+  const float* bank_v;
+  int64_t slots_cap;
+  int k_objects;
+  int64_t slots;
+  const int* dyn_slots;
+  // queries [sets, hw, 128]; object o reads set o / q_div (q_div 0: one set for all objects)
+  const float* qk;
+  int hw, q_div;
+  // output window: 512 channels at out_coff of rows out_cstride wide; HALO rows when halo_w > 0, else row = obj * hw + q
+  void* out;
+  int out_cstride, out_coff, halo_h, halo_w, out_f16;
+};
+
+// The operand checks both entry points share; `who` prefixes the error text.  MIVOS_OK or MIVOS_ERR_INVALID.
+int memread_check_args(const MemreadArgs& a, const char* who);
 
 struct MemreadPlan {
   int algo;
-  int qtile;      // queries per CTA
-  int slot_tile;  // bank slots per inner tile
   int qtiles;
   int splits;  // CTAs along the memory axis
   int nlists;  // candidate lists per (object, query): splits (exact) or splits * kTcHalves (tensor cores)
   int tiles_per_split;
   int kcap;  // list capacity per (object, query, split)
-  // candidate lists are int2 {score bits, slot}: one 8-byte store per append, one load per read
-  int64_t off_list, off_cnt, off_flag, bytes;
+  // candidate lists (int2 {score bits, slot}: one 8-byte store per append, one load per read) start the plan's
+  // workspace, their lengths follow at off_cnt
+  int64_t off_cnt, bytes;
 };
 
 MemreadPlan memread_plan(int k_objects, int64_t slots, int hw, int top_k, int algo);
@@ -39,29 +62,73 @@ MemreadPlan memread_plan(int k_objects, int64_t slots, int hw, int top_k, int al
 // each) start on a 4 KB boundary, so no list straddles a 4 GB boundary and the generator bumps only the low
 // word of its append pointer (the plan reserves the 4 KB of slack).
 inline uint8_t* plan_lists(void* ws, const MemreadPlan& pl) {
-  uint8_t* p = static_cast<uint8_t*>(ws) + pl.off_list;
+  uint8_t* p = static_cast<uint8_t*>(ws);
   if (pl.algo != MIVOS_MEMREAD_TCGEN05) return p;
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 4095) & ~static_cast<uintptr_t>(4095));
 }
 
+// Workspace of the top-k read (byte offsets): the tensor-core plan | the exact plan (fallback) | overflow flags
+// [K*hw] | key-norm maxima [kMaxObjects] | scaled queries [K*hw*128] (one set per object at most; 16-byte aligned:
+// TMA source, float4 stores) | their norms [K*hw] | shared thresholds [K*hw].  The [K*hw] arrays are padded to 256
+// bytes; flags and maxima are adjacent so that one memset clears both.
+struct MemreadWorkspace {
+  MemreadPlan tc, ex;
+  int64_t off_ex, off_overflow, off_kmax2, off_qs, off_qnorm, off_tau, bytes;
+};
+
+MemreadWorkspace memread_workspace(int k_objects, int64_t slots, int hw, int top_k);
+
 // `flags` (optional, [K*hw]): only CTAs owning a flagged query do any work.
-int launch_exact_candidates(const float* bank_k, int64_t slots_cap, int k_objects, int64_t slots,
-                            const float* qk, int hw, int q_div, int top_k, const MemreadPlan& pl, void* ws,
-                            const int* flags, const int* dyn_slots, cudaStream_t stream);
+int launch_exact_candidates(const MemreadArgs& a, int top_k, const MemreadPlan& pl, void* ws, const int* flags,
+                            cudaStream_t stream);
 // Lists come from `pl`/`ws` (approximate scores that need the exact re-score when pl.algo is the tensor-core plan).
 // `flags` (optional, [K*hw]) and `pass`: pass 0 serves the queries whose flag is clear and SETS the flag of a query
 // whose lists hold more in-band candidates than the stage can stage (instead of selecting it); pass 1 serves only
 // the flagged queries (from the exact lists of the fallback).  flags == nullptr: one pass over every query.
-int launch_select(const float* bank_k, const float* bank_v, int64_t slots_cap, int k_objects,
-                  const float* qk, int hw, int q_div, int top_k, const MemreadPlan& pl, void* ws,
-                  const MemreadPlan* fb, void* fb_ws, int* flags, int pass, const float* qnorm,
-                  const float* kmax2, const int* tau_g, void* out, int out_cstride, int out_coff, int halo_h,
-                  int halo_w, int out_f16, int32_t* topk_idx, float* topk_val, cudaStream_t stream);
+int launch_select(const MemreadArgs& a, int top_k, const MemreadPlan& pl, void* ws, int* flags, int pass,
+                  const float* qnorm, const float* kmax2, const int* tau_g, int32_t* topk_idx, float* topk_val,
+                  cudaStream_t stream);
 
-bool memread_tc_available();
-int memread_tc_run(const float* bank_k, const float* bank_v, int64_t slots_cap, int k_objects,
-                   int64_t slots, const float* qk, int hw, int q_div, int top_k, void* out, int out_cstride,
-                   int out_coff, int halo_h, int halo_w, int out_f16, int32_t* topk_idx, float* topk_val,
-                   void* workspace, const int* dyn_slots, cudaStream_t stream);
+int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* topk_val, void* workspace,
+                   cudaStream_t stream);
+
+// float <-> int with the same ordering (so atomicMax on the int is a max on the float)
+__device__ __forceinline__ int float_ordered(float f) {
+  const int b = __float_as_int(f);
+  return b >= 0 ? b : b ^ 0x7fffffff;
+}
+__device__ __forceinline__ float ordered_float(int o) { return __int_as_float(o >= 0 ? o : o ^ 0x7fffffff); }
+
+// Live bank slots: the device-side count when there is one, never more than the capacity (the count indexes the bank).
+__device__ __forceinline__ int64_t live_slots(const int* dyn_slots, int64_t slots, int64_t slots_cap) {
+  const int64_t n = dyn_slots ? static_cast<int64_t>(*dyn_slots) : slots;
+  return n < slots_cap ? n : slots_cap;
+}
+__device__ __forceinline__ int64_t live_slots(const MemreadArgs& a) { return live_slots(a.dyn_slots, a.slots, a.slots_cap); }
+
+// Output row of (object, query) and the store of its 512 read-out channels by one warp: the lane holds the float4
+// pieces lane, lane + 32, lane + 64, lane + 96.
+__device__ __forceinline__ void store_read_row(const MemreadArgs& a, int obj, int q, int lane, const float4 (&v)[4]) {
+  int64_t row;
+  if (a.halo_w > 0) {
+    const int y = q / a.halo_w, x = q - y * a.halo_w;
+    row = (static_cast<int64_t>(obj) * (a.halo_h + 2) + y + 1) * (a.halo_w + 2) + x + 1;
+  } else {
+    row = static_cast<int64_t>(obj) * a.hw + q;
+  }
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int c = (lane + 32 * u) * 4;
+    if (a.out_f16) {
+      const __half2 h01 = __floats2half2_rn(v[u].x, v[u].y), h23 = __floats2half2_rn(v[u].z, v[u].w);
+      uint2 pk;
+      pk.x = *reinterpret_cast<const uint32_t*>(&h01);
+      pk.y = *reinterpret_cast<const uint32_t*>(&h23);
+      *reinterpret_cast<uint2*>(static_cast<__half*>(a.out) + row * a.out_cstride + a.out_coff + c) = pk;
+    } else {
+      *reinterpret_cast<float4*>(static_cast<float*>(a.out) + row * a.out_cstride + a.out_coff + c) = v[u];
+    }
+  }
+}
 
 }  // namespace mivos

@@ -30,7 +30,6 @@
 #include "pdl.cuh"
 #include "memread.h"
 
-#include <cuda_fp16.h>
 #include <atomic>
 
 namespace mivos {
@@ -43,7 +42,6 @@ constexpr int D_THREADS = 256;  // 8 warps
 constexpr int QSTR = 132;       // query / key row stride (floats): conflict-free fragment loads
 constexpr int VSTR = 520;       // value row stride: 520 = 8 mod 32, conflict-free B-fragment loads by slot
 constexpr int PSTR = 36;        // score / P row stride
-constexpr float kSqrtCK = 11.313708498984761f;  // sqrt(128) rounded to fp32, as the reference's divisor
 
 struct DenseSmem {
   float q[DQ][QSTR];        // q / sqrt(128), fp32 (split into hi / lo at fragment load)
@@ -54,12 +52,8 @@ struct DenseSmem {
 };
 
 struct DenseParams {
-  const float* bank_k;
-  const float* bank_v;
-  int64_t slots_cap, slots;
-  const int* dyn_slots;
-  const float* qk;
-  int hw, q_div, chunk_tiles, chunks;
+  MemreadArgs a;
+  int chunk_tiles, chunks;
   float* part_o;   // [K][chunks][hw][512]
   float2* part_ml; // [K][chunks][hw] {m, l}
 };
@@ -98,8 +92,7 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
   const int q0 = blockIdx.x * DQ;
   const int chunk = blockIdx.y;
   const int obj = blockIdx.z;
-  int64_t n_live = p.dyn_slots ? static_cast<int64_t>(*p.dyn_slots) : p.slots;
-  if (n_live > p.slots_cap) n_live = p.slots_cap;
+  const int64_t n_live = live_slots(p.a);
   const int64_t live_tiles = (n_live + DS - 1) / DS;
   const int64_t t_begin = static_cast<int64_t>(chunk) * p.chunk_tiles;
   if (t_begin >= live_tiles) return;  // chunk past the live bank: the combine does not read it
@@ -107,8 +100,8 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
   if (t_end > live_tiles) t_end = live_tiles;
   const int ntiles = static_cast<int>(t_end - t_begin);
 
-  const float* keys = p.bank_k + static_cast<int64_t>(obj) * p.slots_cap * 128;
-  const float* vals = p.bank_v + static_cast<int64_t>(obj) * p.slots_cap * 512;
+  const float* keys = p.a.bank_k + static_cast<int64_t>(obj) * p.a.slots_cap * 128;
+  const float* vals = p.a.bank_v + static_cast<int64_t>(obj) * p.a.slots_cap * 512;
   auto load_tile = [&](int stage, int64_t tile) {
     const int64_t s0 = tile * DS;
     for (int i = tid; i < DS * 32; i += D_THREADS) {  // 32 rows x 32 float4 of keys
@@ -126,11 +119,11 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
   load_tile(0, t_begin);
 
   // query tile, divided by sqrt(128) with the IEEE division of the reference (rows past hw are zero)
-  const float* qk = p.qk + static_cast<int64_t>(p.q_div > 0 ? obj / p.q_div : 0) * p.hw * 128;
+  const float* qk = p.a.qk + static_cast<int64_t>(p.a.q_div > 0 ? obj / p.a.q_div : 0) * p.a.hw * 128;
   for (int i = tid; i < DQ * 32; i += D_THREADS) {
     const int r = i >> 5, c4 = i & 31;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (q0 + r < p.hw) {
+    if (q0 + r < p.a.hw) {
       v = *reinterpret_cast<const float4*>(qk + static_cast<int64_t>(q0 + r) * 128 + c4 * 4);
       v.x = v.x / kSqrtCK; v.y = v.y / kSqrtCK; v.z = v.z / kSqrtCK; v.w = v.w / kSqrtCK;
     }
@@ -255,14 +248,14 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
   }
 
   // ---- partials of this chunk
-  const int64_t prow = (static_cast<int64_t>(obj) * p.chunks + chunk) * p.hw;
-  if (ss == 0 && q0 + sr < p.hw) p.part_ml[prow + q0 + sr] = make_float2(m_run, l_run);
+  const int64_t prow = (static_cast<int64_t>(obj) * p.chunks + chunk) * p.a.hw;
+  if (ss == 0 && q0 + sr < p.a.hw) p.part_ml[prow + q0 + sr] = make_float2(m_run, l_run);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int q = q0 + 16 * i + g + 8 * h;
-      if (q >= p.hw) continue;
+      if (q >= p.a.hw) continue;
       float* dst = p.part_o + (prow + q) * 512 + 64 * warp + 2 * t;
 #pragma unroll
       for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[i][j][2 * h], o[i][j][2 * h + 1]);
@@ -273,18 +266,14 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
 constexpr int C_WARPS = 8;
 
 __global__ void __launch_bounds__(32 * C_WARPS) memread_dense_combine_kernel(
-    const float* __restrict__ part_o, const float2* __restrict__ part_ml, int64_t slots, int64_t slots_cap,
-    const int* __restrict__ dyn_slots,
-    int hw, int chunk_tiles, int chunks, int n_queries, void* __restrict__ out, int out_cstride, int out_coff, int halo_h,
-    int halo_w, int out_f16) {
+    const MemreadArgs a, const float* __restrict__ part_o, const float2* __restrict__ part_ml, int chunk_tiles, int chunks) {
   mivos::pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t lq = static_cast<int64_t>(blockIdx.x) * C_WARPS + warp;  // = obj * hw + q
-  if (lq >= n_queries) return;
+  const int hw = a.hw;
+  if (lq >= static_cast<int64_t>(a.k_objects) * hw) return;
   const int obj = static_cast<int>(lq / hw), q = static_cast<int>(lq - static_cast<int64_t>(obj) * hw);
-  int64_t n_live = dyn_slots ? static_cast<int64_t>(*dyn_slots) : slots;
-  if (n_live > slots_cap) n_live = slots_cap;
-  const int64_t live_tiles = (n_live + DS - 1) / DS;
+  const int64_t live_tiles = (live_slots(a) + DS - 1) / DS;
   const int live = static_cast<int>((live_tiles + chunk_tiles - 1) / chunk_tiles);
   const int64_t base = static_cast<int64_t>(obj) * chunks * hw + q;  // chunk c of this query: base + c * hw
   float M = -INFINITY;
@@ -308,27 +297,9 @@ __global__ void __launch_bounds__(32 * C_WARPS) memread_dense_combine_kernel(
       acc[u].w = fmaf(w, v.w, acc[u].w);
     }
   }
-  int64_t row;
-  if (halo_w > 0) {
-    const int y = q / halo_w, x = q - y * halo_w;
-    row = (static_cast<int64_t>(obj) * (halo_h + 2) + y + 1) * (halo_w + 2) + x + 1;
-  } else {
-    row = lq;
-  }
 #pragma unroll
-  for (int u = 0; u < 4; ++u) {
-    const int c = (lane + 32 * u) * 4;
-    const float4 r = make_float4(acc[u].x / L, acc[u].y / L, acc[u].z / L, acc[u].w / L);
-    if (out_f16) {
-      const __half2 h01 = __floats2half2_rn(r.x, r.y), h23 = __floats2half2_rn(r.z, r.w);
-      uint2 pk;
-      pk.x = *reinterpret_cast<const uint32_t*>(&h01);
-      pk.y = *reinterpret_cast<const uint32_t*>(&h23);
-      *reinterpret_cast<uint2*>(static_cast<__half*>(out) + row * out_cstride + out_coff + c) = pk;
-    } else {
-      *reinterpret_cast<float4*>(static_cast<float*>(out) + row * out_cstride + out_coff + c) = r;
-    }
-  }
+  for (int u = 0; u < 4; ++u) acc[u] = make_float4(acc[u].x / L, acc[u].y / L, acc[u].z / L, acc[u].w / L);
+  store_read_row(a, obj, q, lane, acc);
 }
 
 // Chunk length (tiles of DS slots) as a function of hw alone.  Small frames have few query tiles and need many
@@ -373,18 +344,14 @@ extern "C" MIVOS_API int mivos_memory_read_dense(const float* bank_k, const floa
                                                  int out_halo_w, void* workspace, int64_t workspace_bytes,
                                                  const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  MIVOS_REQUIRE(bank_k && bank_v && qk && out && workspace, "memory_read_dense: null pointer");
+  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
+                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16};
+  const int rc = memread_check_args(a, "memory_read_dense");
+  if (rc != MIVOS_OK) return rc;
   MIVOS_REQUIRE(slots_cap >= 1 && slots_cap < (1ll << 31) - 65536 && slots >= 1 && slots <= slots_cap,
                 "memory_read_dense: bad slot count %lld (cap %lld)", (long long)slots, (long long)slots_cap);
-  MIVOS_REQUIRE(k_objects >= 1 && k_objects <= kMaxObjects && hw >= 1, "memory_read_dense: bad object/query count");
-  MIVOS_REQUIRE(q_div >= 0, "memory_read_dense: q_div must be >= 0 (0: all objects read one query set)");
-  MIVOS_REQUIRE(out_cstride % 4 == 0 && out_coff % 4 == 0 && out_coff >= 0 && out_coff + 512 <= out_cstride,
-                "memory_read_dense: output channel window does not fit");
-  MIVOS_REQUIRE(out_halo_w == 0 || (out_halo_w > 0 && out_halo_h * out_halo_w == hw), "memory_read_dense: halo dims do not match hw");
-  MIVOS_REQUIRE((reinterpret_cast<uintptr_t>(bank_k) & 15) == 0 && (reinterpret_cast<uintptr_t>(bank_v) & 15) == 0 &&
-                    (reinterpret_cast<uintptr_t>(qk) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
-                    (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
-                "memory_read_dense: pointers must be 16-byte aligned (workspace 256)");
+  MIVOS_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
+                "memory_read_dense: workspace null or not 256-byte aligned");
   const DensePlan pl = dense_plan(k_objects, slots_cap, hw);
   MIVOS_REQUIRE(workspace_bytes >= pl.bytes, "memory_read_dense: workspace %lld < %lld bytes", (long long)workspace_bytes,
                 (long long)pl.bytes);
@@ -398,14 +365,7 @@ extern "C" MIVOS_API int mivos_memory_read_dense(const float* bank_k, const floa
   }
   uint8_t* w = static_cast<uint8_t*>(workspace);
   DenseParams p;
-  p.bank_k = bank_k;
-  p.bank_v = bank_v;
-  p.slots_cap = slots_cap;
-  p.slots = slots;
-  p.dyn_slots = dyn_slots;
-  p.qk = qk;
-  p.hw = hw;
-  p.q_div = q_div;
+  p.a = a;
   p.chunk_tiles = pl.chunk_tiles;
   p.chunks = pl.chunks;
   p.part_o = reinterpret_cast<float*>(w);
@@ -414,10 +374,8 @@ extern "C" MIVOS_API int mivos_memory_read_dense(const float* bank_k, const floa
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 
-  const int n_queries = k_objects * hw;
-  launch_pdl(memread_dense_combine_kernel, dim3(ceil_div(n_queries, C_WARPS)), 32 * C_WARPS, 0, stream,
-             static_cast<const float*>(p.part_o), static_cast<const float2*>(p.part_ml), slots, slots_cap, dyn_slots, hw,
-             pl.chunk_tiles, pl.chunks, n_queries, out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16);
+  launch_pdl(memread_dense_combine_kernel, dim3(ceil_div(k_objects * hw, C_WARPS)), 32 * C_WARPS, 0, stream, a,
+             static_cast<const float*>(p.part_o), static_cast<const float2*>(p.part_ml), pl.chunk_tiles, pl.chunks);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;

@@ -36,7 +36,6 @@
 #include "sm90.cuh"
 
 #include <atomic>
-#include <cstdlib>
 
 namespace mivos {
 extern std::atomic<int64_t> g_launches;
@@ -53,9 +52,10 @@ constexpr int STAGE_BYTES = TS * KB * 4;      // 32 KB
 constexpr int WARM = 2;
 constexpr int TC_THREADS = 288;              // 2 MMA / epilogue warpgroups, TMA producer warp
 constexpr int STREAM_CAP = kTcCandCap;        // per (object, query, split) while streaming
-constexpr float kSqrtCK = 11.313708498984761f;
 constexpr float kEpsFactor = kTcMarginFactor;
 
+// The five operand fields the kernel reads, not the whole MemreadArgs: a larger parameter block costs this kernel
+// spills (NB = 32: 334 -> 422 bytes of spill stores per thread with the full block, see the register budget below).
 struct TcParams {
   int64_t slots_cap, slots;
   int hw, top_k, splits, nlists, tiles_per_split;
@@ -68,15 +68,7 @@ struct TcParams {
   int* overflow;        // [K*hw]
   int* tau_g;           // [K*hw] order-preserving int encoding of the best threshold any CTA has found
   int* err;
-  unsigned spin_ns;     // sleep between barrier polls of the TMA / MMA threads (0 = poll flat out)
 };
-
-// float <-> int with the same ordering (so atomicMax on the int is a max on the float)
-__device__ __forceinline__ int float_ordered(float f) {
-  const int b = __float_as_int(f);
-  return b >= 0 ? b : b ^ 0x7fffffff;
-}
-__device__ __forceinline__ float ordered_float(int o) { return __int_as_float(o >= 0 ? o : o ^ 0x7fffffff); }
 
 // ---- prep: scaled queries, their norms, and the max key norm per object --------------------
 __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_rows, int q_div, float* __restrict__ qs,
@@ -85,7 +77,7 @@ __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_
                                     unsigned int* __restrict__ kmax2_bits, int qblocks,
                                     const int* __restrict__ dyn_slots, int* __restrict__ tau_g) {
   mivos::pdl_prologue();
-  if (dyn_slots) slots = *dyn_slots;
+  slots = live_slots(dyn_slots, slots, slots_cap);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (static_cast<int>(blockIdx.x) < qblocks) {
     // one warp per query row r = set * hw + q
@@ -222,7 +214,7 @@ constexpr int STG_BYTES = 64 * STG_STRIDE * 4;
 // each); 9 warps put 3 on one partition, so 16384 / (3 x 32) caps a thread at 168 — a larger cap compiles but the
 // launch is refused.  The 128-float accumulator fragment, the NB bucket maxima and a 32-score chunk do not all fit
 // there: ptxas spills 0.3-1.3 KB per thread (NB = 32 / 64), served from L1, inside the candidate loop.
-template <int NB, bool EMIT_PTX>
+template <int NB>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                   const TcParams p) {
@@ -244,7 +236,7 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const int split = blockIdx.y;
   const int obj = blockIdx.z;
   const int qrow0 = (p.q_div > 0 ? obj / p.q_div : 0) * p.hw;  // first row of this object's query set
-  const int64_t slots = p.dyn_slots ? static_cast<int64_t>(*p.dyn_slots) : p.slots;
+  const int64_t slots = live_slots(p.dyn_slots, p.slots, p.slots_cap);
   const int total_tiles = static_cast<int>((slots + TS - 1) / TS);
   // with a device-side slot count the grid (splits) is fixed by the host for the bank capacity and
   // the tile ranges are derived here; splits beyond the live bank publish empty lists and leave
@@ -295,8 +287,11 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         for (int kb = 0; kb < NKB; ++kb, ++it) {
           const int s = it % STAGES;
           const uint32_t ph = (it / STAGES) & 1;
-          if (p.spin_ns) sm90::mbar_wait_backoff(&empty_bar[s], ph ^ 1, p.err, 301, p.spin_ns);
-          else sm90::mbar_wait(&empty_bar[s], ph ^ 1, p.err, 301);
+          // the first pass over the ring finds every stage free: no sleep there.  (Keeping the two waits also keeps
+          // the register allocation of the epilogue: with the back-off wait alone the NB = 64 kernel measured 6 %
+          // slower at top-k 50 on an H100 at 700 W, with the same register count and fewer spill bytes.)
+          if (it < STAGES) sm90::mbar_wait(&empty_bar[s], ph ^ 1, p.err, 301);
+          else sm90::mbar_wait_backoff(&empty_bar[s], ph ^ 1, p.err, 301, 100);
           sm90::mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
           sm90::tma_load_2d(smem_k + s * STAGE_BYTES, &tmK, &full_bar[s], kb * KB, row);
         }
@@ -397,17 +392,8 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         }
         if (emit) {
           const int idx0 = static_cast<int>(slot0) + col0;
-          if constexpr (EMIT_PTX) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) emit_if_ge(lp, v[j], tau_emit, idx0 + j);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const bool pass = v[j] >= tau_emit;
-              if (pass) *lp = make_int2(__float_as_int(v[j]), idx0 + j);
-              lp += pass ? 1 : 0;
-            }
-          }
+          for (int j = 0; j < 32; ++j) emit_if_ge(lp, v[j], tau_emit, idx0 + j);
         }
       }
     }
@@ -470,102 +456,78 @@ constexpr int TC_SMEM = Q_BYTES + STAGES * STAGE_BYTES + 2 * STG_BYTES + (1 + 2 
 
 }  // namespace
 
-bool memread_tc_available() { return true; }
-
-int memread_tc_run(const float* bank_k, const float* bank_v, int64_t slots_cap, int k_objects,
-                   int64_t slots, const float* qk, int hw, int q_div, int top_k, void* out, int out_cstride,
-                   int out_coff, int halo_h, int halo_w, int out_f16, int32_t* topk_idx, float* topk_val,
-                   void* workspace, const int* dyn_slots, cudaStream_t stream) {
-  MIVOS_REQUIRE(static_cast<int64_t>(k_objects) * slots_cap < (1ll << 31) - 4096,
+int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* topk_val, void* workspace,
+                   cudaStream_t stream) {
+  MIVOS_REQUIRE(static_cast<int64_t>(a.k_objects) * a.slots_cap < (1ll << 31) - 4096,
                 "memory_read(tensor cores): bank rows exceed int32 TMA coordinates");
-  const MemreadPlan tc = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_TCGEN05);
-  const MemreadPlan ex = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
+  const MemreadWorkspace ws = memread_workspace(a.k_objects, a.slots, a.hw, top_k);
+  const MemreadPlan& tc = ws.tc;
   uint8_t* w = static_cast<uint8_t*>(workspace);
-  uint8_t* w_tc = w;
-  uint8_t* w_ex = w + tc.bytes;
-  const int q_sets = q_div > 0 ? ceil_div(k_objects, q_div) : 1;
-  const int q_rows = q_sets * hw;
-  MIVOS_REQUIRE(k_objects <= kMaxObjects, "memory_read: more than %d objects in one call", kMaxObjects);
-  // tail of the workspace (sized for k_objects query sets): flags | key-norm maxima | scaled queries | norms | tau
-  const int64_t nq = static_cast<int64_t>(k_objects) * hw, nq64 = (nq + 63) & ~63ll;  // arrays padded to 256 bytes
-  int* flags = reinterpret_cast<int*>(w + tc.bytes + ex.bytes);
-  unsigned int* kmax2 = reinterpret_cast<unsigned int*>(flags + nq64);
-  float* qs = reinterpret_cast<float*>(kmax2 + kMaxObjects);  // 16-byte aligned: TMA source, float4 stores
-  float* qnorm = qs + nq * 128;
-  int* tau_g = reinterpret_cast<int*>(qnorm + nq64);
+  uint8_t* w_ex = w + ws.off_ex;
+  int* flags = reinterpret_cast<int*>(w + ws.off_overflow);
+  unsigned int* kmax2 = reinterpret_cast<unsigned int*>(w + ws.off_kmax2);
+  float* qs = reinterpret_cast<float*>(w + ws.off_qs);
+  float* qnorm = reinterpret_cast<float*>(w + ws.off_qnorm);
+  int* tau_g = reinterpret_cast<int*>(w + ws.off_tau);
+  const int q_sets = a.q_div > 0 ? ceil_div(a.k_objects, a.q_div) : 1;
+  const int q_rows = q_sets * a.hw;
 
   // overflow flags (written here and by the first selection pass, read by the exact fallback and the second selection
   // pass) and the key-norm accumulator start at zero: ONE memset over the two adjacent arrays
-  MIVOS_CUDA_OK(cudaMemsetAsync(flags, 0, static_cast<size_t>(nq64 + kMaxObjects) * 4, stream));
+  MIVOS_CUDA_OK(cudaMemsetAsync(flags, 0, static_cast<size_t>(ws.off_qs - ws.off_overflow), stream));
 
   const int qblocks = ceil_div(q_rows, 8);
   const int kblocks = 296;
-  launch_pdl(memread_prep_kernel, qblocks + kblocks, 256, 0, stream, qk, hw, q_rows, q_div, qs, qnorm, bank_k, slots_cap, slots,
-                                                             k_objects, kmax2, qblocks, dyn_slots, tau_g);
+  launch_pdl(memread_prep_kernel, qblocks + kblocks, 256, 0, stream, a.qk, a.hw, q_rows, a.q_div, qs, qnorm, a.bank_k,
+             a.slots_cap, a.slots, a.k_objects, kmax2, qblocks, a.dyn_slots, tau_g);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 
   CUtensorMap tmQ, tmK;
   int rc = encode_tmap_2d(&tmQ, qs, static_cast<uint64_t>(q_rows), 128, 128, KB, TQ);
   if (rc != MIVOS_OK) return rc;
-  rc = encode_tmap_2d(&tmK, bank_k, static_cast<uint64_t>(k_objects) * slots_cap, 128, 128, KB, TS);
+  rc = encode_tmap_2d(&tmK, a.bank_k, static_cast<uint64_t>(a.k_objects) * a.slots_cap, 128, 128, KB, TS);
   if (rc != MIVOS_OK) return rc;
 
   TcParams p;
-  p.slots_cap = slots_cap;
-  p.slots = slots;
-  p.dyn_slots = dyn_slots;
-  p.hw = hw;
-  p.q_div = q_div;
+  p.slots_cap = a.slots_cap;
+  p.slots = a.slots;
+  p.dyn_slots = a.dyn_slots;
+  p.hw = a.hw;
+  p.q_div = a.q_div;
   p.top_k = top_k;
   p.splits = tc.splits;
   p.nlists = tc.nlists;
   p.tiles_per_split = tc.tiles_per_split;
   p.qnorm = qnorm;
   p.kmax2 = reinterpret_cast<const float*>(kmax2);
-  p.cand = reinterpret_cast<int2*>(plan_lists(w_tc, tc));
-  p.cand_cnt = reinterpret_cast<int*>(w_tc + tc.off_cnt);
+  p.cand = reinterpret_cast<int2*>(plan_lists(w, tc));
+  p.cand_cnt = reinterpret_cast<int*>(w + tc.off_cnt);
   p.overflow = flags;
   p.tau_g = tau_g;
   p.err = device_error_flag();
 
-  // MIVOS_MEMREAD_EMIT=c selects the compiler's emission loop, MIVOS_MEMREAD_BACKOFF_NS the producer's sleep
-  // between barrier polls (0 = poll flat out)
-  static const bool emit_ptx = [] { const char* e = getenv("MIVOS_MEMREAD_EMIT"); return !(e && e[0] == 'c'); }();
-  static const unsigned spin_ns = [] { const char* e = getenv("MIVOS_MEMREAD_BACKOFF_NS"); return e ? static_cast<unsigned>(atoi(e)) : 100u; }();
-  p.spin_ns = spin_ns;
-
   static bool configured = false;
   if (!configured) {
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
     configured = true;
   }
-  dim3 grid(tc.qtiles, tc.splits, k_objects);
-  if (top_k <= 32) {
-    if (emit_ptx) launch_pdl(memread_tc_kernel<32, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-    else launch_pdl(memread_tc_kernel<32, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-  } else {
-    if (emit_ptx) launch_pdl(memread_tc_kernel<64, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-    else launch_pdl(memread_tc_kernel<64, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-  }
+  dim3 grid(tc.qtiles, tc.splits, a.k_objects);
+  if (top_k <= 32) launch_pdl(memread_tc_kernel<32>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  else launch_pdl(memread_tc_kernel<64>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 
   // selection pass A: every query the candidate pass did not flag, from the tensor-core lists; a query whose lists carry
   // more in-band candidates than the stage can hold is flagged there instead of being selected
-  rc = launch_select(bank_k, bank_v, slots_cap, k_objects, qk, hw, q_div, top_k, tc, w_tc, nullptr, nullptr, flags, 0, qnorm,
-                     reinterpret_cast<const float*>(kmax2), tau_g, out, out_cstride, out_coff, halo_h, halo_w, out_f16, topk_idx,
-                     topk_val, stream);
+  rc = launch_select(a, top_k, tc, w, flags, 0, qnorm, p.kmax2, tau_g, topk_idx, topk_val, stream);
   if (rc != MIVOS_OK) return rc;
   // exact fallback for flagged queries only (CTAs without a flagged query exit immediately) ...
-  rc = launch_exact_candidates(bank_k, slots_cap, k_objects, slots, qk, hw, q_div, top_k, ex, w_ex, flags, dyn_slots, stream);
+  rc = launch_exact_candidates(a, top_k, ws.ex, w_ex, flags, stream);
   if (rc != MIVOS_OK) return rc;
   // ... and selection pass B: the flagged queries, from the exact lists (warps of the others leave at once)
-  return launch_select(bank_k, bank_v, slots_cap, k_objects, qk, hw, q_div, top_k, ex, w_ex, nullptr, nullptr, flags, 1, nullptr,
-                       nullptr, nullptr, out, out_cstride, out_coff, halo_h, halo_w, out_f16, topk_idx, topk_val, stream);
+  return launch_select(a, top_k, ws.ex, w_ex, flags, 1, nullptr, nullptr, nullptr, topk_idx, topk_val, stream);
 }
 
 }  // namespace mivos

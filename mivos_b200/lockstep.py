@@ -26,7 +26,6 @@ import torch
 
 from . import _lib, ops, schedule
 from ._lib import MivosError
-from .engine import QueryState
 from .inference_core import InferenceCore
 
 
@@ -101,8 +100,6 @@ class _LockStep:
         if visible * self.hw < self.net.min_live_slots:  # same rule as the eager path (mivos_memory_read) and torch.topk
             raise MivosError(f"memory_read: {visible * self.hw} live bank slots < top_k {self.net.top_k}")
         C, K = self.C, self.K
-        if isinstance(cached, QueryState):  # the C clips' states of this frame, contiguous (joint query pass)
-            cached = [_clip_view(cached, c) for c in range(C)]
         srcs, dsts = [], []
         for c in range(C):
             q = cached[c]
@@ -129,79 +126,6 @@ class _LockStep:
         return self.prob
 
 
-def _rows(qs: QueryState, a: int, b: int) -> QueryState:
-    """Images [a, b) of a batched QueryState (views)."""
-    return QueryState(kv=qs.kv[a:b], qk=qs.qk[a:b], s8=qs.s8[a:b], s4=qs.s4[a:b], h=qs.h, w=qs.w)
-
-
-def _clip_view(qs: QueryState, c: int) -> QueryState:
-    """Clip c of a batched QueryState in the shape InferenceCore caches per-clip states (qk [hw,128])."""
-    return QueryState(kv=qs.kv[c:c + 1], qk=qs.qk[c], s8=qs.s8[c:c + 1], s4=qs.s4[c:c + 1], h=qs.h, w=qs.w)
-
-
-class _JointQueryCache:
-    """Query-side features of the lock-step clips, computed CHUNK frames x C clips at a time in ONE
-    batched pass on the side stream (instead of one pass of CHUNK frames per clip), frame-major
-    (image f*C + c), so that the C states of a frame are one contiguous block: the step stages them
-    with 4 copies instead of 4*C.  Same caching rule as InferenceCore.get_query_kv_buffered
-    (reference inference_core.py:110-120): a frame index is encoded once and kept until the cache
-    exceeds q_buf_size frames, then flushed wholesale.  A/B option (MIVOS_LOCKSTEP_JOINT_QUERY=1)."""
-
-    def __init__(self, cores: Sequence[InferenceCore]):
-        self.cores = list(cores)
-        c0 = cores[0]
-        self.C, self.t, self.nh, self.nw = len(cores), c0.t, c0.nh, c0.nw
-        self.q_buf_size = c0.q_buf_size
-        if c0.mem_profile > 1:
-            raise MivosError("the joint query pass keeps a chunk of staged frames alive: mem_profile 0 or 1 only")
-        self.chunk = max(1, min(InferenceCore.QUERY_CHUNK, self.q_buf_size))
-        self.eng = c0.prop_net.engine()
-        self.stream = c0._qstream
-        self.device = c0.device
-        self.buf = {}     # frame idx -> (QueryState of the C clips, ready event)
-        self.pool = []    # batched allocations of chunk*C states, recycled across flushes
-        self.live = []
-
-    def _issue(self, want):
-        n, C = len(want), self.C
-        entry = self.pool.pop() if self.pool else self.eng.new_query_states(self.nh, self.nw, self.chunk * C)[1]
-        batch = entry if n == self.chunk else _rows(entry, 0, n * C)
-        frames = torch.stack([core.get_image_buffered(j)[0] for j in want for core in self.cores], 0)  # frame-major
-        cur = torch.cuda.current_stream(self.device)
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            self.cores[0].prop_net.encode_query_batch_resident(frames, batch)
-            ready = torch.cuda.Event()
-            ready.record(self.stream)
-        frames.record_stream(self.stream)
-        self.live.append(entry)
-        for f, j in enumerate(want):
-            self.buf[j] = (_rows(entry, f * C, (f + 1) * C), ready)
-
-    def get(self, idx: int, step: int, stop: Optional[int]) -> QueryState:
-        lookahead = 2 * self.chunk if self.q_buf_size >= 2 * InferenceCore.QUERY_CHUNK else 1
-        j, covered = idx, 0
-        while covered < lookahead and 0 <= j < self.t and (stop is None or j != stop):
-            if j in self.buf:
-                j += step
-                covered += 1
-                continue
-            if len(self.buf) > self.q_buf_size and j == idx:
-                self.pool.extend(self.live)
-                self.buf, self.live = {}, []
-            want = []
-            while len(want) < self.chunk and 0 <= j < self.t and (stop is None or j != stop):
-                if j not in self.buf:
-                    want.append(j)
-                j += step
-            covered += len(want)
-            want.sort()
-            self._issue(want)
-        qs, ready = self.buf[idx]
-        torch.cuda.current_stream(self.device).wait_event(ready)
-        return qs
-
-
 class LockstepSession:
     def __init__(self, cores: Sequence[InferenceCore]):
         if len(cores) < 1:
@@ -218,7 +142,6 @@ class LockstepSession:
         # passes must be stream-ordered among themselves, so they all run on the first clip's side stream
         for c in cores[1:]:
             c._qstream = c0._qstream
-        self.joint = _JointQueryCache(self.cores) if os.environ.get("MIVOS_LOCKSTEP_JOINT_QUERY", "0") == "1" else None
 
     def interact(self, masks: Sequence[torch.Tensor], idx: int, total_cb=None, step_cb=None) -> List[np.ndarray]:
         """C x InferenceCore.interact(mask_c, idx).  `total_cb(n)` / `step_cb()` count frames per clip
@@ -247,12 +170,7 @@ class LockstepSession:
             step.bank_v[o, :num_certain * hw].copy_(core._certain_bank_v)
         for fp in plan.frames:
             ti = fp.ti
-            if self.joint is not None:
-                joint = self.joint.get(ti, plan.step, plan.closest_ti)
-                cached = [_clip_view(joint, c) for c in range(C)]
-            else:
-                joint = None
-                cached = [core.get_query_kv_buffered(ti, plan.step, plan.closest_ti) for core in cores]
+            cached = [core.get_query_kv_buffered(ti, plan.step, plan.closest_ti) for core in cores]
             # the step stages its operands and (unless the frames are fused) writes every clip's prob[:, ti] itself
             frames = [core.get_image_buffered(ti) for core in cores] if fp.memorize else [None] * C
             prob = step.run(frames, cached, fp.visible, fp.m_front, fp.memorize,

@@ -347,6 +347,23 @@ def memory_read_workspace_bytes(k: int, slots: int, hw: int, top_k: int) -> int:
     return int(n)
 
 
+def _memread_operands(who: str, bank_k, bank_v, qk, out, q_div: int, halo_hw, workspace, need_bytes):
+    """What memory_read and memory_read_dense share: operand and query-set checks, (k, cap, hw), a workspace of at
+    least need_bytes(k, cap, hw) bytes, and the halo dims ((0, 0): pixel-major output)."""
+    _req(bank_k), _req(bank_v), _req(qk), _req_act(out)
+    k, cap = bank_k.shape[0], bank_k.shape[1]
+    hw = qk.shape[-2]
+    if qk.dim() == 3 and (q_div < 1 or (k + q_div - 1) // q_div != qk.shape[0]):
+        raise _lib.MivosError(f"{who}: {qk.shape[0]} query sets for {k} objects need q_div = objects per set (got {q_div})")
+    if qk.dim() == 2 and q_div != 0:
+        raise _lib.MivosError(f"{who}: q_div needs a [sets,hw,128] query tensor")
+    need = need_bytes(k, cap, hw)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=qk.device)
+    hh, ww = halo_hw if halo_hw is not None else (0, 0)
+    return k, cap, hw, workspace, hh, ww
+
+
 def memory_read(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, top_k: int,
                 out: torch.Tensor, *, out_coff: int = 0, halo_hw=None, workspace: Optional[torch.Tensor] = None,
                 algo: int = MEMREAD_AUTO, want_topk: bool = False, dyn_slots: Optional[torch.Tensor] = None,
@@ -354,21 +371,13 @@ def memory_read(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torc
     """bank_k [K,cap,128], bank_v [K,cap,512], qk pixel-major [hw,128] — or [sets,hw,128] with q_div objects
     per query set (object o reads set o // q_div: the C clips of a lock-step step in ONE call).  `out` is a
     HALO map (pass halo_hw=(h,w)) or pixel-major [K,hw,C]."""
-    _req(bank_k), _req(bank_v), _req(qk), _req_act(out)
-    k, cap = bank_k.shape[0], bank_k.shape[1]
-    hw = qk.shape[-2]
-    if qk.dim() == 3 and (q_div < 1 or (k + q_div - 1) // q_div != qk.shape[0]):
-        raise _lib.MivosError(f"memory_read: {qk.shape[0]} query sets for {k} objects need q_div = objects per set (got {q_div})")
-    if qk.dim() == 2 and q_div != 0:
-        raise _lib.MivosError("memory_read: q_div needs a [sets,hw,128] query tensor")
-    need = memory_read_workspace_bytes(k, slots, hw, top_k)
-    if workspace is None or workspace.numel() < need:
-        workspace = torch.empty(need, dtype=torch.uint8, device=qk.device)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read", bank_k, bank_v, qk, out, q_div, halo_hw, workspace,
+        lambda k, cap, hw: memory_read_workspace_bytes(k, slots, hw, top_k))
     idx = val = None
     if want_topk:
         idx = torch.empty((k, hw, top_k), dtype=torch.int32, device=qk.device)
         val = torch.empty((k, hw, top_k), dtype=torch.float32, device=qk.device)
-    hh, ww = halo_hw if halo_hw is not None else (0, 0)
     check(_lib.lib().mivos_memory_read(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, q_div, top_k, _ptr(out),
                                        out.shape[-1], out_coff, hh, ww, _ptr(idx), _ptr(val), _ptr(workspace),
                                        workspace.numel(), algo, _ptr(dyn_slots), _f16(out), _stream()),
@@ -389,17 +398,8 @@ def memory_read_dense(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk
                       dyn_slots: Optional[torch.Tensor] = None, q_div: int = 0):
     """The reference's dense read (EvalMemoryReader with top_k=None): softmax over all `slots` live bank slots.
     Operands, query sets (q_div), output window and dyn_slots as for memory_read."""
-    _req(bank_k), _req(bank_v), _req(qk), _req_act(out)
-    k, cap = bank_k.shape[0], bank_k.shape[1]
-    hw = qk.shape[-2]
-    if qk.dim() == 3 and (q_div < 1 or (k + q_div - 1) // q_div != qk.shape[0]):
-        raise _lib.MivosError(f"memory_read_dense: {qk.shape[0]} query sets for {k} objects need q_div = objects per set (got {q_div})")
-    if qk.dim() == 2 and q_div != 0:
-        raise _lib.MivosError("memory_read_dense: q_div needs a [sets,hw,128] query tensor")
-    need = memory_read_dense_workspace_bytes(k, cap, hw)
-    if workspace is None or workspace.numel() < need:
-        workspace = torch.empty(need, dtype=torch.uint8, device=qk.device)
-    hh, ww = halo_hw if halo_hw is not None else (0, 0)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_dense", bank_k, bank_v, qk, out, q_div, halo_hw, workspace, memory_read_dense_workspace_bytes)
     check(_lib.lib().mivos_memory_read_dense(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, q_div, _ptr(out),
                                              out.shape[-1], out_coff, hh, ww, _ptr(workspace), workspace.numel(),
                                              _ptr(dyn_slots), _f16(out), _stream()),

@@ -50,14 +50,38 @@ def _call(lib, **kw):
                                        p(a["ws"]), a["ws_bytes"], p(a["dyn"]), a["f16"], p(0))
 
 
-@pytest.mark.parametrize("bad", [dict(bank_k=0), dict(slots=0), dict(slots=101), dict(k=0), dict(k=257), dict(hw=0),
-                                 dict(q_div=-1), dict(cstride=510), dict(coff=4), dict(hh=3, hw_=4),
-                                 dict(bank_v=260), dict(ws=272), dict(ws_bytes=1024)])
+BAD_OPERANDS = [dict(bank_k=0), dict(slots=0), dict(slots=101), dict(k=0), dict(k=257), dict(hw=0),
+                dict(q_div=-1), dict(cstride=510), dict(coff=4), dict(hh=3, hw_=4),
+                dict(bank_v=260), dict(ws=272), dict(ws_bytes=1024)]
+
+
+@pytest.mark.parametrize("bad", BAD_OPERANDS)
 def test_dense_read_rejects_bad_arguments_before_any_device_call(bad):
     from mivos_b200 import _lib
     lib = _lib.load()
     assert _call(lib, **bad) == -1
     assert lib.mivos_last_error().decode().startswith("memory_read_dense")
+
+
+def _call_topk(lib, **kw):
+    a = dict(bank_k=256, bank_v=256, slots_cap=100, k=1, slots=50, qk=256, hw=10, q_div=0, top_k=20, out=256,
+             cstride=512, coff=0, hh=0, hw_=0, ws=256, ws_bytes=1 << 40, algo=0, dyn=None, f16=0)
+    a.update(kw)
+    p = lambda v: C.c_void_p(v)  # noqa: E731  (never dereferenced: the checks come first)
+    return lib.mivos_memory_read(p(a["bank_k"]), p(a["bank_v"]), a["slots_cap"], a["k"], a["slots"], p(a["qk"]), a["hw"],
+                                 a["q_div"], a["top_k"], p(a["out"]), a["cstride"], a["coff"], a["hh"], a["hw_"], p(None),
+                                 p(None), p(a["ws"]), a["ws_bytes"], a["algo"], p(a["dyn"]), a["f16"], p(0))
+
+
+@pytest.mark.parametrize("bad", BAD_OPERANDS + [dict(cstride=1024, coff=-4), dict(qk=260), dict(top_k=0), dict(top_k=65),
+                                                dict(algo=7)])
+def test_topk_read_rejects_bad_arguments_before_any_device_call(bad):
+    """The top-k read checks its operands by the rules of the dense read: a window that starts before the row
+    (out_coff < 0) and a query pointer its kernels could not load as float4 are argument errors, not launches."""
+    from mivos_b200 import _lib
+    lib = _lib.load()
+    assert _call_topk(lib, **bad) == -1
+    assert lib.mivos_last_error().decode().startswith("memory_read:")
 
 
 def test_dense_network_surface():

@@ -174,31 +174,6 @@ def test_reset_gives_the_state_of_a_new_session(rt, golden):
         assert torch.equal(core.prob, p1) and (m1b == m1).all()
 
 
-@pytest.mark.parametrize("mem_profile", [0, 1])
-def test_lockstep_joint_query_pass_is_an_equivalent_schedule(rt, monkeypatch, mem_profile):
-    """MIVOS_LOCKSTEP_JOINT_QUERY=1: the query-side features of the lock-step clips come from ONE batched
-    pass of chunk x C frames (frame-major) instead of C passes; results are those of the default path."""
-    from oracle import weights as Wt
-    mv, net, fuse = rt
-    C, K, T = 2, 1, 12  # 11 propagated frames: two chunks of 8, the second one short
-    clips = [Wt.synthetic_clip(T, 64, 96, K, seed=60 + i) for i in range(C)]
-    masks = [m for _, m in clips]
-    masks2 = [m.flip(-2).contiguous() for m in masks]
-    res = {}
-    for joint in ("0", "1"):
-        monkeypatch.setenv("MIVOS_LOCKSTEP_JOINT_QUERY", joint)
-        cores = [mv.InferenceCore(net, fuse, img, K, mem_profile=mem_profile, mem_freq=3, device="cpu") for img, _ in clips]
-        sess = mv.LockstepSession(cores)
-        assert (sess.joint is not None) == (joint == "1")
-        o1 = [o.copy() for o in sess.interact(masks, 0)]
-        o2 = sess.interact(masks2, 11)  # backward pass over cached frames, fused
-        res[joint] = (o1, o2, [c.prob.clone() for c in cores], [list(c.bank_trace) for c in cores])
-    for c in range(C):
-        assert res["0"][3][c] == res["1"][3][c]
-        assert float((res["0"][2][c] - res["1"][2][c]).abs().max()) <= 1e-4
-        assert (res["0"][0][c] == res["1"][0][c]).mean() >= 0.9999 and (res["0"][1][c] == res["1"][1][c]).mean() >= 0.9999
-
-
 def test_cfg1_480p_host_runtime_matches_reference_masks(rt, golden):
     """BASELINE configs[0] (480p 5-frame clip, 1 object, 3-frame memory) through the host runtime over
     the emulated operators: the DAVIS shape (854 -> 864 padding, 30x54 key maps, 1620-slot bank frames)."""
