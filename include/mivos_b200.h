@@ -233,6 +233,21 @@ MIVOS_API int mivos_memory_read_dense(const float* bank_k, const float* bank_v, 
                       void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
                       void* workspace, int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
                       mivos_stream_t stream);
+/* Wide top-k memory read — EvalMemoryReader.forward + softmax_w_g_top (prop_net.py:47-73, 81-108) for
+ * 1 <= top_k <= 1024: the semantics of mivos_memory_read (exact fp32 scores, total order score desc /
+ * slot asc, softmax over the k survivors, read-out in ascending slot order) and, for top_k <= 64, its
+ * bits.  Operands, query sets, output window, dyn_slots and topk_idx / topk_val as for
+ * mivos_memory_read; top_k <= slots <= slots_cap.  Scores are exact fp32 on CUDA cores: two histogram
+ * sweeps find each query's threshold, a third emits the candidates, one CTA per query sorts them
+ * (ties and near-ties beyond a query's candidate region: an exact radix select in that CTA).
+ * `workspace` sized by mivos_memory_read_wide_workspace() (it depends on k_objects and hw alone;
+ * 256-byte aligned); returns -1 on bad arguments.                                                  */
+MIVOS_API int64_t mivos_memory_read_wide_workspace(int k_objects, int64_t slots_cap, int hw, int top_k);
+MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int q_div, int top_k,
+                      void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
+                      const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
 /* Diagnostic, synchronising: candidate statistics of the last tensor-core-path read in `workspace`:
  * out[0] total candidates, out[1] max per (object, query), out[2] queries served by the exact
  * fallback, out[3] splits of the memory axis.                                                    */

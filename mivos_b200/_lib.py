@@ -86,6 +86,8 @@ SIGNATURES = {
     "mivos_memory_read_stats": (_i, [_p, _i, _l, _i, _i, C.POINTER(_l)]),
     "mivos_memory_read_dense_workspace": (_l, [_i, _l, _i]),
     "mivos_memory_read_dense": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _i, _i, _i, _p, _l, _p, _i, _p]),
+    "mivos_memory_read_wide_workspace": (_l, [_i, _l, _i, _i]),
+    "mivos_memory_read_wide": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _p, _i, _p]),
     "mivos_upsample4x_sigmoid_aggregate": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p]),
     "mivos_aggregate_wbg": (_i, [_p, _i, _l, _i, _i, _p, _p]),
     "mivos_argmax_unpad": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p]),

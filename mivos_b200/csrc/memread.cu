@@ -217,19 +217,6 @@ constexpr int B_THREADS = 32 * kSelWarps;
 constexpr int B_MAXSURV = kSelMaxSurvivors;  // candidates (staged) / survivors (re-scored) one query may hold
 constexpr int kSelBytesPerWarp = B_MAXSURV * 8 + 128 * 4 + MAXK * 16 + (kMaxLists + 1) * 4 + 28;
 
-__device__ __forceinline__ float exact_score(const float* __restrict__ key, const float* qs) {
-  float acc = 0.f;
-#pragma unroll 16
-  for (int c4 = 0; c4 < 32; ++c4) {
-    const float4 kv = *reinterpret_cast<const float4*>(key + c4 * 4);
-    acc = fmaf(kv.x, qs[c4 * 4 + 0], acc);
-    acc = fmaf(kv.y, qs[c4 * 4 + 1], acc);
-    acc = fmaf(kv.z, qs[c4 * 4 + 2], acc);
-    acc = fmaf(kv.w, qs[c4 * 4 + 3], acc);
-  }
-  return acc;
-}
-
 struct SelectLists {
   const int2* e;  // {score bits, slot}
   const int* cnt;

@@ -1,4 +1,5 @@
-// Internal interface between the memory-read translation units (memread.cu, memread_tc.cu, memread_dense.cu):
+// Internal interface between the memory-read translation units (memread.cu, memread_tc.cu, memread_dense.cu,
+// memread_wide.cu):
 // the operands of a read, the workspace layout of the top-k read, and the device pieces the kernels share.
 #pragma once
 #include "host_util.h"
@@ -105,6 +106,21 @@ __device__ __forceinline__ int64_t live_slots(const int* dyn_slots, int64_t slot
   return n < slots_cap ? n : slots_cap;
 }
 __device__ __forceinline__ int64_t live_slots(const MemreadArgs& a) { return live_slots(a.dyn_slots, a.slots, a.slots_cap); }
+
+// The exact score of one key row against a scaled query (q / sqrt(128)): fmaf in ascending channel order.  Every
+// read that selects slots ranks them by this value.  The chain starts at +0, so it never yields -0.
+__device__ __forceinline__ float exact_score(const float* __restrict__ key, const float* qs) {
+  float acc = 0.f;
+#pragma unroll 16
+  for (int c4 = 0; c4 < 32; ++c4) {
+    const float4 kv = *reinterpret_cast<const float4*>(key + c4 * 4);
+    acc = fmaf(kv.x, qs[c4 * 4 + 0], acc);
+    acc = fmaf(kv.y, qs[c4 * 4 + 1], acc);
+    acc = fmaf(kv.z, qs[c4 * 4 + 2], acc);
+    acc = fmaf(kv.w, qs[c4 * 4 + 3], acc);
+  }
+  return acc;
+}
 
 // Output row of (object, query) and the store of its 512 read-out channels by one warp: the lane holds the float4
 // pieces lane, lane + 32, lane + 64, lane + 96.

@@ -18,6 +18,7 @@ from typing import Dict, Optional, Tuple
 import torch
 
 from . import arch, ops
+from ._lib import MivosError
 from .ops import PackedConv
 
 BN_EPS = 1e-5
@@ -361,13 +362,21 @@ class PropagationEngine(_ResNetTrunk):
         return 1 if self.top_k is None else self.top_k
 
     def _memory_read(self, bank_k, bank_v, slots: int, qk, n: int, cat, h16: int, w16: int, dyn_slots, q_div: int):
-        """The memory read of n objects into channels [0, 512) of `cat`: the top-k read (prop_net.py:47-73), or
-        the dense read of the reference's top_k=None (prop_net.py:99-102).  The only place that tells them apart."""
+        """The memory read of n objects into channels [0, 512) of `cat`: the top-k read (prop_net.py:47-73) for
+        top_k <= 64, the wide top-k read above that, or the dense read of the reference's top_k=None
+        (prop_net.py:99-102).  The only place that tells them apart."""
         hw = h16 * w16
         if self.top_k is None:
             wsp = self.ws.raw("memread_dense", ops.memory_read_dense_workspace_bytes(n, bank_k.shape[1], hw))
             ops.memory_read_dense(bank_k, bank_v, slots, qk, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
                                   dyn_slots=dyn_slots, q_div=q_div)
+        elif self.top_k > ops.TOPK_READ_MAX_K:
+            if self.top_k > ops.WIDE_READ_MAX_K:
+                raise MivosError(f"memory read: top_k {self.top_k} exceeds the largest served top_k "
+                                 f"({ops.WIDE_READ_MAX_K})")
+            wsp = self.ws.raw("memread_wide", ops.memory_read_wide_workspace_bytes(n, bank_k.shape[1], hw, self.top_k))
+            ops.memory_read_wide(bank_k, bank_v, slots, qk, self.top_k, cat, out_coff=0, halo_hw=(h16, w16),
+                                 workspace=wsp, dyn_slots=dyn_slots, q_div=q_div)
         else:
             wsp = self.ws.raw("memread", ops.memory_read_workspace_bytes(n, slots, hw, self.top_k))
             ops.memory_read(bank_k, bank_v, slots, qk, self.top_k, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,

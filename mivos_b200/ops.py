@@ -348,7 +348,7 @@ def memory_read_workspace_bytes(k: int, slots: int, hw: int, top_k: int) -> int:
 
 
 def _memread_operands(who: str, bank_k, bank_v, qk, out, q_div: int, halo_hw, workspace, need_bytes):
-    """What memory_read and memory_read_dense share: operand and query-set checks, (k, cap, hw), a workspace of at
+    """What memory_read, memory_read_dense and memory_read_wide share: operand and query-set checks, (k, cap, hw), a workspace of at
     least need_bytes(k, cap, hw) bytes, and the halo dims ((0, 0): pixel-major output)."""
     _req(bank_k), _req(bank_v), _req(qk), _req_act(out)
     k, cap = bank_k.shape[0], bank_k.shape[1]
@@ -405,6 +405,40 @@ def memory_read_dense(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk
                                              _ptr(dyn_slots), _f16(out), _stream()),
           "mivos_memory_read_dense")
     return out
+
+
+TOPK_READ_MAX_K = 64     # memory_read
+WIDE_READ_MAX_K = 1024   # memory_read_wide
+
+
+def memory_read_wide_workspace_bytes(k: int, slots_cap: int, hw: int, top_k: int) -> int:
+    """Workspace of memory_read_wide for k objects (it depends on k and hw alone)."""
+    n = _lib.load().mivos_memory_read_wide_workspace(k, slots_cap, hw, top_k)
+    if n < 0:
+        raise _lib.MivosError(f"memory_read_wide_workspace: bad arguments (k={k} slots_cap={slots_cap} hw={hw} "
+                              f"top_k={top_k}; 1 <= top_k <= {WIDE_READ_MAX_K})")
+    return int(n)
+
+
+def memory_read_wide(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, top_k: int,
+                     out: torch.Tensor, *, out_coff: int = 0, halo_hw=None, workspace: Optional[torch.Tensor] = None,
+                     want_topk: bool = False, dyn_slots: Optional[torch.Tensor] = None, q_div: int = 0):
+    """The top-k read for 1 <= top_k <= 1024 (the reference's EvalMemoryReader with any top_k), with the semantics
+    of memory_read and, for top_k <= 64, its bits.  Operands, query sets (q_div), output window and dyn_slots as for
+    memory_read."""
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_wide", bank_k, bank_v, qk, out, q_div, halo_hw, workspace,
+        lambda k, cap, hw: memory_read_wide_workspace_bytes(k, cap, hw, top_k))
+    idx = val = None
+    if want_topk:
+        idx = torch.empty((k, hw, top_k), dtype=torch.int32, device=qk.device)
+        val = torch.empty((k, hw, top_k), dtype=torch.float32, device=qk.device)
+    check(_lib.lib().mivos_memory_read_wide(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, q_div, top_k,
+                                            _ptr(out), out.shape[-1], out_coff, hh, ww, _ptr(idx), _ptr(val),
+                                            _ptr(workspace), workspace.numel(), _ptr(dyn_slots), _f16(out),
+                                            _stream()),
+          "mivos_memory_read_wide")
+    return (out, idx, val) if want_topk else out
 
 
 def upsample4x_sigmoid_aggregate(logits: torch.Tensor, k: int, h4: int, w4: int, coff: int = 0,
