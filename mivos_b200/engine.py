@@ -12,6 +12,7 @@ Reference semantics followed (paths relative to the reference root):
 """
 from __future__ import annotations
 
+import contextlib
 from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
 
@@ -217,23 +218,17 @@ class PropagationEngine(_ResNetTrunk):
         self._pack(state_dict)
         self.memread_algo = ops.MEMREAD_AUTO
 
+    @contextlib.contextmanager
     def lane(self, i: int):
         """Context manager: the sequential-step workspace of lane i becomes `self.ws` (eager launches and graph
         CAPTURE bind buffer addresses; replay does not touch the engine)."""
-        eng = self
-
-        class _Lane:
-            def __enter__(self_inner):
-                if i not in eng._ws_lanes:
-                    eng._ws_lanes[i] = Workspace(eng.device, eng.act_dtype)
-                self_inner.prev = eng.ws
-                eng.ws = eng._ws_lanes[i]
-
-            def __exit__(self_inner, *exc):
-                eng.ws = self_inner.prev
-                return False
-
-        return _Lane()
+        if i not in self._ws_lanes:
+            self._ws_lanes[i] = Workspace(self.device, self.act_dtype)
+        prev, self.ws = self.ws, self._ws_lanes[i]
+        try:
+            yield
+        finally:
+            self.ws = prev
 
     # ------------------------------------------------------------------ packing
     def _pack(self, sd):
@@ -328,17 +323,20 @@ class PropagationEngine(_ResNetTrunk):
         self.encode_query_batch(frame.reshape(1, 3, H, W), qs)
         return qs
 
-    def encode_memory(self, frame: torch.Tensor, masks: torch.Tensor) -> torch.Tensor:
-        """memorize (prop_net.py:144-162): returns the HALO [K,H/16,W/16,640] key|value map
-        (a workspace buffer: consume before the next call)."""
-        K, _, H, W = masks.shape
+    def encode_memory(self, frames: torch.Tensor, masks: torch.Tensor) -> torch.Tensor:
+        """memorize (prop_net.py:144-162) of one clip (frame [1,3,H,W], masks [K,1,H,W]) or of C clips (frames
+        [C,3,H,W], masks [C,K,1,H,W], any clip stride): returns the HALO [C*K,H/16,W/16,640] key|value map, clip-major
+        (a workspace buffer: consume before the next call).  The "others" channel sums over the objects of the SAME
+        clip: the stem gather takes the C (frame, K masks) groups in one launch."""
+        H, W = masks.shape[-2:]
+        N = masks.shape[:-3].numel()  # K, or C*K
         pcs = self.pc["mask_rgb_encoder.conv1"]
-        stem = self.ws.mat("stem_m", K * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
-        ops.stem_gather(frame.reshape(1, 3, H, W), masks, stem, s2d=True)
-        f16 = self._trunk("mask_rgb_encoder", arch.MASK_LAYERS, stem, K, H, W, {}, self.ws)
+        stem = self.ws.mat("stem_m", N * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
+        ops.stem_gather(frames.reshape(-1, 3, H, W), masks, stem, s2d=True)
+        f16 = self._trunk("mask_rgb_encoder", arch.MASK_LAYERS, stem, N, H, W, {}, self.ws)
         h16, w16 = H // 16, W // 16
-        kv = self.ws.halo("kv_m", K, h16, w16, 640, torch.float32)
-        _cg(self.ws, f16, self.pc["kv_m_f16"], K, h16, w16, kv)
+        kv = self.ws.halo("kv_m", N, h16, w16, 640, torch.float32)
+        _cg(self.ws, f16, self.pc["kv_m_f16"], N, h16, w16, kv)
         return kv
 
     # ------------------------------------------------------------------ decoder
@@ -382,31 +380,37 @@ class PropagationEngine(_ResNetTrunk):
             ops.memory_read(bank_k, bank_v, slots, qk, self.top_k, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
                             algo=self.memread_algo, dyn_slots=dyn_slots, q_div=q_div)
 
-    def segment(self, bank_k, bank_v, slots: int, qs: QueryState, K: int, *, want_raw=False, want_prob=True,
-                prob_out=None, dyn_slots=None):
-        """segment_with_query (prop_net.py:170-181) + aggregate_wbg(keep_bg=True)
-        (inference_core.py:175).  Returns (raw sigmoid [K,1,H,W] | None, prob [(K+1),1,H,W] | None)."""
+    def segment(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int = 1, *, prob_out=None, want_raw=False,
+                want_prob=True, dyn_slots=None):
+        """segment_with_query (prop_net.py:170-181) + aggregate_wbg(keep_bg=True) (inference_core.py:175) for C
+        clips.  The C*K object maps (clip-major: map c*K + k is object k of clip c) go through every convolution as
+        ONE batch — the 1/16- and 1/8-resolution layers of a single clip have 14-54 row tiles for 132 SMs — while the
+        operators whose operands differ per clip (memory read, skip broadcast, aggregation) take the C clips as groups
+        of one launch.  bank_k/bank_v [C*K, cap, 128/512]; `q` the QueryState of one clip's frame, or for C > 1 the
+        batched state of the C current frames (new_query_states(H, W, C)).  Returns (raw sigmoid [C*K,1,H,W] | None,
+        prob [(K+1),1,H,W] | None), prob [C,K+1,1,H,W] for C > 1."""
         ws, pc = self.ws, self.pc
-        H, W = qs.h, qs.w
+        H, W = q.h, q.w
         h16, w16 = H // 16, W // 16
-        hw = h16 * w16
-        cat = ws.halo("cat", K, h16, w16, 1024)
-        self._memory_read(bank_k, bank_v, slots, qs.qk, K, cat, h16, w16, dyn_slots, 0)
-        ops.halo_copy(qs.kv, cat, K, h16, w16, 512, src_coff=128, dst_coff=512)  # cat([readout, v16]) :178-179
-        catr = ws.halo("catr", K, h16, w16, 1024)
-        ops.halo_copy(cat, catr, K, h16, w16, 1024, relu=True)
-        x16 = ws.halo("dec16", K, h16, w16, 512)
-        self._resblock("decoder.compress", cat, catr, K, h16, w16, 1024, 512, x16)
-        # up_16_8 / up_8_4 (modules.py:100-104): the skip paths were produced by the query pass
-        # (qs.s8 / qs.s4, batch 1); the reference broadcasts them over the objects in the add
-        x8 = ws.halo("dec8", K, H // 8, W // 8, 256)
-        self._upblock_tail("decoder.up_16_8", qs.s8, x16, K, H // 8, W // 8, 512, 256, x8, final_relu=False)
-        x4 = ws.halo("dec4", K, H // 4, W // 4, 256)
-        self._upblock_tail("decoder.up_8_4", qs.s4, x8, K, H // 4, W // 4, 256, 256, x4, final_relu=True)
-        lg = ws.halo("logit", K, H // 4, W // 4, 32, torch.float32)
-        _cg(ws, x4, pc["decoder.pred"], K, H // 4, W // 4, lg)
+        N = C * K
+        cat = ws.halo("cat", N, h16, w16, 1024)
+        # ONE read for the C clips: object c*K + k reads query set c (q_div = K objects per set; one clip: q_div 0)
+        self._memory_read(bank_k, bank_v, slots, q.qk, N, cat, h16, w16, dyn_slots, K if C > 1 else 0)
+        ops.halo_copy(q.kv, cat, N, h16, w16, 512, src_coff=128, dst_coff=512)  # cat([readout, v16]) :178-179
+        catr = ws.halo("catr", N, h16, w16, 1024)
+        ops.halo_copy(cat, catr, N, h16, w16, 1024, relu=True)
+        x16 = ws.halo("dec16", N, h16, w16, 512)
+        self._resblock("decoder.compress", cat, catr, N, h16, w16, 1024, 512, x16)
+        # up_16_8 / up_8_4 (modules.py:100-104): the skip paths were produced by the query pass (q.s8 / q.s4, one map
+        # per clip); the reference broadcasts them over the objects in the add
+        x8 = ws.halo("dec8", N, H // 8, W // 8, 256)
+        self._upblock_tail("decoder.up_16_8", q.s8, x16, N, H // 8, W // 8, 512, 256, x8, final_relu=False)
+        x4 = ws.halo("dec4", N, H // 4, W // 4, 256)
+        self._upblock_tail("decoder.up_8_4", q.s4, x8, N, H // 4, W // 4, 256, 256, x4, final_relu=True)
+        lg = ws.halo("logit", N, H // 4, W // 4, 32, torch.float32)
+        _cg(ws, x4, pc["decoder.pred"], N, H // 4, W // 4, lg)
         return ops.upsample4x_sigmoid_aggregate(lg, K, H // 4, W // 4, want_raw=want_raw, want_prob=want_prob,
-                                                prob_out=prob_out)
+                                                prob_out=prob_out, groups=C)
 
     def _upblock_tail(self, p, s2_skip, up, K, h, w, up_c, out_c, out, final_relu):
         """x = skip (one map per frame, broadcast over that frame's objects) + bilinear_x2(up); out_conv ResBlock."""
@@ -415,55 +419,6 @@ class PropagationEngine(_ResNetTrunk):
         s2r = ws.halo("ub_s2r", K, h, w, up_c)
         ops.upsample2x_add(s2, up, K, h, w, x_relu=s2r, skip=s2_skip)
         return self._resblock(f"{p}.out_conv", s2, s2r, K, h, w, up_c, out_c, out, out_relu_only=final_relu)
-
-
-    # ------------------------------------------------------------------ lock-step multi-clip step
-    # C independent clips advance one frame per call as ONE batch of C*K maps through every
-    # convolution (row tiles per launch x C: the 1/16- and 1/8-resolution layers of a single clip
-    # have 14-54 row tiles for 132 SMs).  The operators whose operands differ per clip — the memory
-    # read (own bank, own query), the skip-path broadcast, the stem gather and the aggregation over a
-    # clip's objects — take the C clips as groups of ONE launch (query sets / skip_n / groups of the C ABI).
-    # Object maps are clip-major: image c*K + k is object k of clip c.
-    def segment_multi(self, bank_k, bank_v, slots: int, qb: QueryState, K: int, C: int, prob_out: torch.Tensor,
-                      dyn_slots=None) -> torch.Tensor:
-        """segment() for C clips: bank_k/bank_v [C*K, cap, 128/512], qb the batched QueryState of the C
-        current frames (new_query_states(H, W, C)), prob_out [C, K+1, 1, H, W]."""
-        ws, pc = self.ws, self.pc
-        H, W = qb.h, qb.w
-        h16, w16 = H // 16, W // 16
-        hw = h16 * w16
-        N = C * K
-        cat = ws.halo("cat", N, h16, w16, 1024)
-        # ONE read for the C clips: object c*K + k reads query set c (q_div = K objects per set)
-        self._memory_read(bank_k, bank_v, slots, qb.qk, N, cat, h16, w16, dyn_slots, K)
-        ops.halo_copy(qb.kv, cat, N, h16, w16, 512, src_coff=128, dst_coff=512)  # clip c's v16 over its K objects
-        catr = ws.halo("catr", N, h16, w16, 1024)
-        ops.halo_copy(cat, catr, N, h16, w16, 1024, relu=True)
-        x16 = ws.halo("dec16", N, h16, w16, 512)
-        self._resblock("decoder.compress", cat, catr, N, h16, w16, 1024, 512, x16)
-        # the C frames' skip paths (qb.s8 / qb.s4: one map per clip) are broadcast over each clip's K objects
-        x8 = ws.halo("dec8", N, H // 8, W // 8, 256)
-        self._upblock_tail("decoder.up_16_8", qb.s8, x16, N, H // 8, W // 8, 512, 256, x8, final_relu=False)
-        x4 = ws.halo("dec4", N, H // 4, W // 4, 256)
-        self._upblock_tail("decoder.up_8_4", qb.s4, x8, N, H // 4, W // 4, 256, 256, x4, final_relu=True)
-        lg = ws.halo("logit", N, H // 4, W // 4, 32, torch.float32)
-        _cg(ws, x4, pc["decoder.pred"], N, H // 4, W // 4, lg)
-        ops.upsample4x_sigmoid_aggregate(lg, K, H // 4, W // 4, prob_out=prob_out, groups=C)
-        return prob_out
-
-    def encode_memory_multi(self, frames: torch.Tensor, masks: torch.Tensor) -> torch.Tensor:
-        """encode_memory() for C clips: frames [C,3,H,W], masks [C,K,1,H,W] (any clip stride) -> HALO
-        [C*K,H/16,W/16,640] key|value map (a workspace buffer).  The "others" channel sums over the objects
-        of the SAME clip: the stem gather takes the C (frame, K masks) groups in one launch."""
-        C, K, _, H, W = masks.shape
-        pcs = self.pc["mask_rgb_encoder.conv1"]
-        stem = self.ws.mat("stem_m", C * K * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
-        ops.stem_gather(frames, masks, stem, s2d=True)
-        f16 = self._trunk("mask_rgb_encoder", arch.MASK_LAYERS, stem, C * K, H, W, {}, self.ws)
-        h16, w16 = H // 16, W // 16
-        kv = self.ws.halo("kv_m", C * K, h16, w16, 640, torch.float32)
-        _cg(self.ws, f16, self.pc["kv_m_f16"], C * K, h16, w16, kv)
-        return kv
 
 
 class FusionEngine:

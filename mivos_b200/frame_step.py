@@ -1,0 +1,128 @@
+"""The per-frame step of the propagation loop, for one clip (``InferenceCore``) or for C clips that advance
+together (``LockstepSession``): a single clip is the case C = 1."""
+from __future__ import annotations
+
+import weakref
+from typing import Optional, Sequence
+
+import torch
+
+from . import _lib, ops
+from ._lib import MivosError
+
+
+class FrameStep:
+    """One propagated frame of C clips (memory read -> decoder -> aggregate [-> memorize trunk -> bank write]) as a
+    captured CUDA graph.  The C*K object maps go through every convolution as ONE batch (C times the row tiles per
+    launch); the operators whose operands differ per clip take the C clips as groups of one launch
+    (engine.PropagationEngine.segment / encode_memory).  Everything that changes from frame to frame lives in device
+    memory the graph reads: each clip's frame and query-side features (from its batched query pass,
+    InferenceCore.get_query_kv_buffered) are staged into `frames[c]` / `batch`, the live bank size and the bank slot of
+    the memorize are the int32 scalars `dyn` (identical for all clips: they execute one plan), results land in
+    `prob[c]`.  One graph with and one without the memorize serve every frame of every pass while the bank grows, so
+    the kernel launches of a frame cost one graph launch on the host.  Instances (with their bank buffers) are
+    cached on the network's engine and shared by successive sessions — the reference also shares the networks between
+    sessions (eval_interactive_davis.py:83)."""
+
+    def __init__(self, net, C: int, K: int, nh: int, nw: int, cap_frames: int, lane: int = 0):
+        eng = net.engine()
+        dev = eng.device
+        # the step is cached on the network's engine: a strong reference back would be a cycle that keeps a dropped
+        # network's workspaces, banks and graphs in device memory until the garbage collector happens to run
+        self.net = weakref.proxy(net)
+        self.C, self.K, self.nh, self.nw, self.lane = C, K, nh, nw, lane
+        self.hw = (nh // 16) * (nw // 16)
+        self.cap_frames = cap_frames
+        self.frames = torch.zeros((C, 3, nh, nw), dtype=torch.float32, device=dev)
+        self.prob = torch.zeros((C, K + 1, 1, nh, nw), dtype=torch.float32, device=dev)
+        self.dyn = torch.zeros(4, dtype=torch.int32, device=dev)
+        states, self.batch = eng.new_query_states(nh, nw, C)
+        # one clip keeps the single-clip operands: [hw,128] query keys (read without query sets), [K+1,1,H,W] planes
+        self.q, self.out = (states[0], self.prob[0]) if C == 1 else (self.batch, self.prob)
+        self.masks = self.out.narrow(-4, 1, K)  # the object planes the memorize reads
+        self.bank_k = torch.empty((C * K, cap_frames * self.hw, 128), dtype=torch.float32, device=dev)
+        self.bank_v = torch.empty((C * K, cap_frames * self.hw, 512), dtype=torch.float32, device=dev)
+        self.graphs = {}
+        self.kernels = {}  # kernels per replay, for mivos_launch_count accounting
+        # False: eager launches even when the caller asks for graph replay (bench.py's per-launch brackets)
+        self.use_graph = True
+        # Device pointer table of the step (mivos_copy_segments): the graph STAGES each clip's operands itself — frame,
+        # cached query features kv / qk / s8 / s4: source pointers in dynp[:5C] — and DELIVERS its K+1 result planes to
+        # InferenceCore.prob[:, ti] (destination pointers in dynp[5C:]); per frame the host writes the table and the two
+        # bank counters with ONE small launch (mivos_store_words) and replays the graph: no eager copy.
+        b = self.batch
+        staged = [t for c in range(C) for t in (self.frames[c], b.kv[c], b.qk[c], b.s8[c], b.s4[c])]
+        i64 = lambda v: torch.tensor(v, dtype=torch.int64, device=dev)  # noqa: E731
+        self.g_fixed = i64([t.data_ptr() for t in staged])
+        self.g_bytes_host = [t.numel() * t.element_size() for t in staged]
+        self.g_bytes = i64(self.g_bytes_host)
+        self.s_fixed = i64([self.prob[c, j].data_ptr() for c in range(C) for j in range(K + 1)])
+        self.plane_bytes = nh * nw * 4
+        self.s_bytes = i64([self.plane_bytes] * (C * (K + 1)))
+        self.dynp = torch.zeros(C * (6 + K), dtype=torch.int64, device=dev)
+
+    @staticmethod
+    def get(net, C: int, K: int, nh: int, nw: int, need_frames: int, lane: int = 0) -> "FrameStep":
+        """The cached step for these shapes.  Single clips are kept in the engine's `_frame_steps` (4 entries),
+        lock-step groups, whose C*K banks are C times larger, in `_lock_steps` (2 entries); least recently used
+        first out."""
+        name, bound = ("_frame_steps", 4) if C == 1 else ("_lock_steps", 2)
+        cache = net.engine().__dict__.setdefault(name, {})
+        cap = (need_frames + 15) // 16 * 16
+        key = (C, K, nh, nw, cap, lane)
+        step = cache.pop(key, None)
+        if step is None:
+            step = FrameStep(net, C, K, nh, nw, cap, lane)
+            while len(cache) >= bound:  # dict order = use order
+                cache.pop(next(iter(cache)))
+        cache[key] = step  # (re)insert as most recently used
+        return step
+
+    def _body(self, memorize: bool):
+        eng, C, K = self.net.engine(), self.C, self.K
+        with eng.lane(self.lane):
+            ops.copy_segments(self.g_fixed, self.dynp, self.g_bytes, 5 * C, True, max(self.g_bytes_host))
+            eng.segment(self.bank_k, self.bank_v, self.cap_frames * self.hw, self.q, K, C, prob_out=self.out,
+                        dyn_slots=self.dyn[0:1])
+            if memorize:
+                kv = eng.encode_memory(self.frames, self.masks)
+                # the C*K object banks are contiguous and share the frame slot: one launch
+                ops.bank_write(kv, C * K, self.nh // 16, self.nw // 16, 0, 128, self.bank_k, self.bank_v,
+                               self.cap_frames - 1, dyn_t=self.dyn[1:2])
+            ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, C * (K + 1), False, self.plane_bytes)
+
+    def run(self, frames: Sequence[Optional[torch.Tensor]], cached, visible: int, m_front: int, memorize: bool,
+            prob_dsts=None, ti: int = 0, graph: bool = True) -> torch.Tensor:
+        """`frames[c]` [1,3,nh,nw] (device; read when memorizing) and `cached[c]` the QueryState of clip c's frame;
+        `prob_dsts[c]` [(K+1),T,1,nh,nw]: the step writes clip c's result planes to prob_dsts[c][:, ti] itself (None:
+        they are only left in self.prob[c], e.g. for fuse_one_frame).  `graph`: replay the captured graph (the
+        calling session's use_graph), else launch eagerly.  Returns self.prob [C,K+1,1,nh,nw]."""
+        assert visible <= self.cap_frames and m_front < self.cap_frames
+        if visible * self.hw < self.net.min_live_slots:  # same rule as mivos_memory_read and torch.topk
+            raise MivosError(f"memory_read: {visible * self.hw} live bank slots < top_k {self.net.top_k}")
+        srcs, dsts = [], []
+        for c in range(self.C):
+            q = cached[c]
+            srcs += [frames[c].data_ptr() if memorize else 0, q.kv.data_ptr(), q.qk.data_ptr(), q.s8.data_ptr(),
+                     q.s4.data_ptr()]
+            dsts += [prob_dsts[c][j, ti].data_ptr() for j in range(self.K + 1)] if prob_dsts is not None else [0] * (self.K + 1)
+        ops.store_words(self.dynp, srcs + dsts, self.dyn, (visible * self.hw, m_front))
+        if not (graph and self.use_graph):
+            self._body(memorize)
+            return self.prob
+        lib = _lib.load()
+        g = self.graphs.get(memorize)
+        if g is None:
+            # first use: run eagerly once (allocates every workspace, sets kernel attributes), then capture
+            n0 = lib.mivos_launch_count()
+            self._body(memorize)
+            self.kernels[memorize] = lib.mivos_launch_count() - n0
+            torch.cuda.current_stream().synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._body(memorize)
+            lib.mivos_add_launch_count(-self.kernels[memorize])  # capture issued no work
+            self.graphs[memorize] = g
+        g.replay()
+        lib.mivos_add_launch_count(self.kernels[memorize])
+        return self.prob

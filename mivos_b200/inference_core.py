@@ -26,103 +26,8 @@ import os
 
 from . import _lib, ops, schedule
 from .engine import QueryState
+from .frame_step import FrameStep
 from .tensor_util import pad_divide_by
-
-
-class _FrameStep:
-    """One propagated frame (query encoder -> memory read -> decoder -> aggregate [-> memorize]) as
-    a captured CUDA graph.  Everything that changes from frame to frame lives in device memory the
-    graph reads: the frame is staged into `frame`, the live bank size and the bank slot of the
-    memorize are the int32 scalars `dyn` (mivos_store_i32 writes them from launch arguments), the
-    result lands in `prob`.  The query-side features of the frame come from the batched query pass
-    (InferenceCore.get_query_kv_buffered) and are staged into `qs`.  One graph with and one
-    without the memorize serve every frame of
-    every pass while the bank grows, so the ~130 kernel launches of a frame cost one graph launch
-    on the host.  Instances (with their bank buffers) are cached on the network's engine, keyed by
-    (objects, padded size, bank capacity), and shared by successive InferenceCore objects — the
-    reference also shares the networks between sessions (eval_interactive_davis.py:83)."""
-
-    def __init__(self, net, K: int, nh: int, nw: int, cap_frames: int, lane: int = 0):
-        eng = net.engine()
-        dev = eng.device
-        self.net, self.K, self.nh, self.nw, self.lane = net, K, nh, nw, lane
-        self.hw = (nh // 16) * (nw // 16)
-        self.cap_frames = cap_frames
-        self.frame = torch.zeros((1, 3, nh, nw), dtype=torch.float32, device=dev)
-        self.prob = torch.zeros((K + 1, 1, nh, nw), dtype=torch.float32, device=dev)
-        self.dyn = torch.zeros(4, dtype=torch.int32, device=dev)
-        self.qs = eng.new_query_state(nh, nw)
-        self.bank_k = torch.empty((K, cap_frames * self.hw, 128), dtype=torch.float32, device=dev)
-        self.bank_v = torch.empty((K, cap_frames * self.hw, 512), dtype=torch.float32, device=dev)
-        self.graphs = {}
-        self.kernels = {}  # kernels per replay, for mivos_launch_count accounting
-        # Device pointer table of the step (mivos_copy_segments): the graph STAGES the frame's operands itself —
-        # frame, cached query features kv / qk / s8 / s4: source pointers in dynp[0:5] — and DELIVERS the K+1 result
-        # planes to InferenceCore.prob[:, ti] (destination pointers in dynp[5:]); per frame the host writes the table
-        # and the two bank counters with ONE small launch (mivos_store_words) and replays the graph: no eager copy.
-        staged = [self.frame, self.qs.kv, self.qs.qk, self.qs.s8, self.qs.s4]
-        i64 = lambda v: torch.tensor(v, dtype=torch.int64, device=dev)  # noqa: E731
-        self.g_fixed = i64([t.data_ptr() for t in staged])
-        self.g_bytes_host = [t.numel() * t.element_size() for t in staged]
-        self.g_bytes = i64(self.g_bytes_host)
-        self.s_fixed = i64([self.prob[j].data_ptr() for j in range(K + 1)])
-        self.plane_bytes = nh * nw * 4
-        self.s_bytes = i64([self.plane_bytes] * (K + 1))
-        self.dynp = torch.zeros(5 + K + 1, dtype=torch.int64, device=dev)
-
-    MAX_CACHED = 4  # step objects (bank + query staging + graphs) kept per network, least recently used first out
-
-    @staticmethod
-    def get(net, K, nh, nw, need_frames, lane: int = 0):
-        eng = net.engine()
-        cache = eng.__dict__.setdefault("_frame_steps", {})
-        cap = (need_frames + 15) // 16 * 16
-        key = (K, nh, nw, cap, lane)
-        step = cache.pop(key, None)
-        if step is None:
-            step = _FrameStep(net, K, nh, nw, cap, lane)
-            while len(cache) >= _FrameStep.MAX_CACHED:  # evict the least recently used entry (dict order = use order)
-                cache.pop(next(iter(cache)))
-        cache[key] = step  # (re)insert as most recently used
-        return step
-
-    def _body(self, memorize: bool):
-        net = self.net
-        with net.engine().lane(self.lane):
-            ops.copy_segments(self.g_fixed, self.dynp, self.g_bytes, 5, True, max(self.g_bytes_host))
-            net.segment_resident(self.bank_k, self.bank_v, self.cap_frames * self.hw, self.qs, self.K, prob_out=self.prob,
-                                 dyn_slots=self.dyn[0:1])
-            if memorize:
-                net.memorize_resident(self.frame, self.prob[1:], self.bank_k, self.bank_v, self.cap_frames - 1,
-                                      dyn_slot=self.dyn[1:2])
-            ops.copy_segments(self.s_fixed, self.dynp[5:], self.s_bytes, self.K + 1, False, self.plane_bytes)
-
-    def run(self, frame, qs_cached: QueryState, visible_frames: int, m_front: int, memorize: bool, prob_dst=None, ti: int = 0):
-        """`frame` [1,3,nh,nw] and `qs_cached` on the device; `prob_dst` [(K+1),T,1,nh,nw]: the step writes its result
-        planes to prob_dst[:, ti] itself (None: the result is only left in self.prob, e.g. for fuse_one_frame)."""
-        assert visible_frames <= self.cap_frames and m_front < self.cap_frames
-        if visible_frames * self.hw < self.net.min_live_slots:  # same rule as the eager path (mivos_memory_read) and torch.topk
-            raise _lib.MivosError(f"memory_read: {visible_frames * self.hw} live bank slots < top_k {self.net.top_k}")
-        srcs = [frame.data_ptr() if memorize else 0, qs_cached.kv.data_ptr(), qs_cached.qk.data_ptr(),
-                qs_cached.s8.data_ptr(), qs_cached.s4.data_ptr()]
-        dsts = [prob_dst[j, ti].data_ptr() for j in range(self.K + 1)] if prob_dst is not None else [0] * (self.K + 1)
-        ops.store_words(self.dynp, srcs + dsts, self.dyn, (visible_frames * self.hw, m_front))
-        g = self.graphs.get(memorize)
-        if g is None:
-            # first use: run eagerly once (allocates every workspace, sets kernel attributes), then capture
-            lib = _lib.load()
-            n0 = lib.mivos_launch_count()
-            self._body(memorize)
-            self.kernels[memorize] = lib.mivos_launch_count() - n0
-            torch.cuda.current_stream().synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._body(memorize)
-            lib.mivos_add_launch_count(-self.kernels[memorize])  # capture issued no work
-            self.graphs[memorize] = g
-        g.replay()
-        _lib.load().mivos_add_launch_count(self.kernels[memorize])
-        return self.prob, self.qs
 
 
 class InferenceCore:
@@ -204,12 +109,10 @@ class InferenceCore:
         self.certain_mem_v = None
         self._certain_bank_k = None  # BANK layout [K, n*hw16, 128]
         self._certain_bank_v = None
-        self._bank_k = None
-        self._bank_v = None
         self._masks_unpadded = torch.zeros((t, h, w), dtype=torch.uint8, device=self.device)
         self._fuse_planes = None
         self.bank_trace = []  # (frame, visible bank frames) per propagated frame, for plumbing tests
-        # CUDA-graph replay of the per-frame step (MIVOS_GRAPH=0 falls back to eager launches)
+        # CUDA-graph replay of the per-frame step (MIVOS_GRAPH=0: the step's launches are issued eagerly)
         self.use_graph = os.environ.get("MIVOS_GRAPH", "1") != "0"
         # forward and backward pass of one interaction as two concurrent lanes (MIVOS_BIDIR=0: one after the other)
         self.overlap_passes = os.environ.get("MIVOS_BIDIR", "1") != "0"
@@ -306,58 +209,8 @@ class InferenceCore:
         return self.query_buf[idx]
 
     # ------------------------------------------------------------------ one pass (:122-200)
-    def _pass_setup(self, idx, forward, lane: int = 0):
-        """Plan of one pass (:128-141), its frame-step object / bank (lane 0 or 1), certain memories copied in
-        (:146-151)."""
-        K, hw = self.k, self.hw16
-        num_certain = self._certain_bank_k.shape[1] // hw
-        # the bank bookkeeping of the pass (:128-141, :166-186) is host arithmetic: schedule.plan_pass
-        plan = schedule.plan_pass(self.t, self.interacted, idx, forward, self.mem_freq, num_certain)
-        step = None
-        if not plan.frames:
-            return plan, None, None, None
-        if self.use_graph:
-            # bank sized for the longest pass of this clip plus a fixed interaction budget, so the bank
-            # pointers (and with them the captured graphs) stay valid across passes and sessions
-            step = _FrameStep.get(self.prop_net, K, self.nh, self.nw,
-                                  schedule.bank_capacity_frames(self.t, self.mem_freq, num_certain, plan.total_m), lane)
-            bank_k, bank_v = step.bank_k, step.bank_v
-        else:
-            need = plan.total_m * hw
-            if self._bank_k is None or self._bank_k.shape[1] < need:
-                self._bank_k = torch.empty((K, need, 128), dtype=torch.float32, device=self.device)
-                self._bank_v = torch.empty((K, need, 512), dtype=torch.float32, device=self.device)
-            bank_k, bank_v = self._bank_k, self._bank_v
-        bank_k[:, :num_certain * hw].copy_(self._certain_bank_k)
-        bank_v[:, :num_certain * hw].copy_(self._certain_bank_v)
-        return plan, step, bank_k, bank_v
-
-    def _pass_frame(self, plan, step, bank_k, bank_v, fp, key_k, idx, trace):
-        """One propagated frame of a pass (:165-194) on the current stream."""
-        K, hw, ti = self.k, self.hw16, fp.ti
-        trace.append((ti, fp.visible))
-        qs = self.get_query_kv_buffered(ti, plan.step, plan.closest_ti)  # :172
-        if step is not None:
-            # the graph stages the operands and (unless the frame is fused) writes prob[:, ti] itself  # :173-179, :194
-            frame = self.get_image_buffered(ti) if fp.memorize else None
-            out_mask, qs = step.run(frame, qs, fp.visible, fp.m_front, fp.memorize,
-                                    prob_dst=None if plan.fuse else self.prob, ti=ti)
-        else:
-            _, out_mask = self.prop_net.segment_resident(bank_k, bank_v, fp.visible * hw, qs, K)  # :173-175
-            if fp.memorize:  # :177-179
-                self.prop_net.memorize_resident(self.get_image_buffered(ti), out_mask[1:], bank_k, bank_v, fp.m_front)
-        if plan.fuse:  # :190-194
-            self.prob[:, ti] = self.fuse_one_frame(plan.closest_ti, idx, ti, self.prob[:, ti], out_mask, key_k, qs)
-        elif step is None:
-            self.prob[:, ti] = out_mask
-
     def do_pass(self, key_k, key_v, idx, forward=True, step_cb=None):
-        plan, step, bank_k, bank_v = self._pass_setup(idx, forward)
-        for fp in plan.frames:
-            self._pass_frame(plan, step, bank_k, bank_v, fp, key_k, idx, self.bank_trace)
-            if step_cb is not None:
-                step_cb()
-        return plan.closest_ti
+        return run_pass([self], [key_k], idx, forward, step_cb)
 
     def _do_passes_overlapped(self, key_k, key_v, idx, step_cb=None):
         """The forward and the backward pass of one interaction are independent until the argmax
@@ -366,8 +219,8 @@ class InferenceCore:
         pass fill the SMs the other's latency-bound chain leaves idle.  Each pass executes exactly the
         launches of do_pass in the same order: results are bit-identical to the sequential passes.
         bank_trace keeps the reference's order (all forward frames, then all backward frames)."""
-        pf = self._pass_setup(idx, True, lane=0)
-        pb = self._pass_setup(idx, False, lane=1)
+        pf = _pass_setup([self], idx, True, lane=0)
+        pb = _pass_setup([self], idx, False, lane=1)
         cur = torch.cuda.current_stream(self.device)
         if self._lane_stream is None:
             self._lane_stream = torch.cuda.Stream(device=self.device)
@@ -378,12 +231,12 @@ class InferenceCore:
         nf, nb = len(pf[0].frames), len(pb[0].frames)
         for i in range(max(nf, nb)):
             if i < nf:
-                self._pass_frame(*pf, pf[0].frames[i], key_k, idx, tf)
+                _pass_frame([self], *pf, pf[0].frames[i], [key_k], idx, [tf])
                 if step_cb is not None:
                     step_cb()
             if i < nb:
                 with torch.cuda.stream(side):
-                    self._pass_frame(*pb, pb[0].frames[i], key_k, idx, tb)
+                    _pass_frame([self], *pb, pb[0].frames[i], [key_k], idx, [tb])
                 if step_cb is not None:
                     step_cb()
         cur.wait_stream(side)
@@ -510,3 +363,51 @@ class InferenceCore:
         self.masks[idx] = mp[0]
         self.np_masks[idx] = mo[0].cpu().numpy()
         return self.np_masks
+
+
+# ---------------------------------------------------------------------- the pass loop, for one clip or C lock-step clips
+def run_pass(cores, keys, idx, forward, step_cb=None):
+    """One pass (:122-200) of every clip of `cores` (InferenceCore objects that share one pass plan: one clip, or
+    the clips of a LockstepSession) from the interacted frame `idx`; keys[c]: clip c's interacted key in BANK
+    layout.  step_cb() once per frame of the pass.  Returns the frame that bounds the pass."""
+    plan, step = _pass_setup(cores, idx, forward)
+    for fp in plan.frames:
+        _pass_frame(cores, plan, step, fp, keys, idx, [core.bank_trace for core in cores])
+        if step_cb is not None:
+            step_cb()
+    return plan.closest_ti
+
+
+def _pass_setup(cores, idx, forward, lane: int = 0):
+    """Plan of one pass (:128-141), the frame step that serves it (lane 0 or 1) and every clip's certain memories
+    copied into its banks (:146-151)."""
+    c0 = cores[0]
+    K, hw = c0.k, c0.hw16
+    num_certain = c0._certain_bank_k.shape[1] // hw
+    # the bank bookkeeping of the pass (:128-141, :166-186) is host arithmetic: schedule.plan_pass
+    plan = schedule.plan_pass(c0.t, c0.interacted, idx, forward, c0.mem_freq, num_certain)
+    if not plan.frames:
+        return plan, None
+    # bank sized for the longest pass of this clip plus a fixed interaction budget, so the bank
+    # pointers (and with them the captured graphs) stay valid across passes and sessions
+    step = FrameStep.get(c0.prop_net, len(cores), K, c0.nh, c0.nw,
+                         schedule.bank_capacity_frames(c0.t, c0.mem_freq, num_certain, plan.total_m), lane)
+    for c, core in enumerate(cores):
+        step.bank_k[c * K:(c + 1) * K, :num_certain * hw].copy_(core._certain_bank_k)
+        step.bank_v[c * K:(c + 1) * K, :num_certain * hw].copy_(core._certain_bank_v)
+    return plan, step
+
+
+def _pass_frame(cores, plan, step, fp, keys, idx, traces):
+    """One propagated frame of a pass (:165-194) for every clip, on the current stream.  The first core's use_graph
+    decides between graph replay and eager launches."""
+    ti = fp.ti
+    cached = [core.get_query_kv_buffered(ti, plan.step, plan.closest_ti) for core in cores]  # :172
+    # the step stages its operands and (unless the frame is fused) writes every clip's prob[:, ti] itself  # :173-179, :194
+    frames = [core.get_image_buffered(ti) if fp.memorize else None for core in cores]
+    prob = step.run(frames, cached, fp.visible, fp.m_front, fp.memorize,
+                    prob_dsts=None if plan.fuse else [core.prob for core in cores], ti=ti, graph=cores[0].use_graph)
+    for c, core in enumerate(cores):
+        traces[c].append((ti, fp.visible))
+        if plan.fuse:  # :190-194
+            core.prob[:, ti] = core.fuse_one_frame(plan.closest_ti, idx, ti, core.prob[:, ti], prob[c], keys[c], cached[c])

@@ -105,19 +105,13 @@ class PropagationNetwork(nn.Module):
         self.engine().encode_query_batch(self._f32(frames), batch)
 
     def memorize_resident(self, frame: torch.Tensor, masks: torch.Tensor, bank_k: torch.Tensor, bank_v: torch.Tensor,
-                          slot: int, dyn_slot: Optional[torch.Tensor] = None) -> None:
-        """memorize() straight into BANK slot `slot` (slot-major keys/values).  `dyn_slot`: int32
-        device scalar that overrides `slot` at run time (CUDA-graph replay)."""
+                          slot: int) -> None:
+        """memorize() straight into BANK slot `slot` (slot-major keys/values)."""
         eng = self.engine()
         masks = self._f32(masks)
         K, _, H, W = masks.shape
         kv = eng.encode_memory(self._f32(frame), masks)
-        ops.bank_write(kv, K, H // 16, W // 16, 0, 128, bank_k, bank_v, slot, dyn_t=dyn_slot)
-
-    def segment_resident(self, bank_k, bank_v, slots: int, qs: QueryState, K: int, want_raw=False, want_prob=True,
-                         prob_out=None, dyn_slots=None):
-        return self.engine().segment(bank_k, bank_v, slots, qs, K, want_raw=want_raw, want_prob=want_prob,
-                                     prob_out=prob_out, dyn_slots=dyn_slots)
+        ops.bank_write(kv, K, H // 16, W // 16, 0, 128, bank_k, bank_v, slot)
 
     # ------------------------------------------------------------------ reference-layout API
     def memorize(self, frame: torch.Tensor, masks: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def test_bracketed_pass_and_roofline_dicts(monkeypatch, prop_sd):
+def test_bracketed_pass_over_the_frame_step_and_roofline_dicts(monkeypatch, prop_sd):
     import bench
     from oracle import weights as Wt
     mv = abi_emulator.install_host_runtime(monkeypatch)
@@ -33,13 +33,13 @@ def test_bracketed_pass_and_roofline_dicts(monkeypatch, prop_sd):
     assert os.environ["MIVOS_GRAPH"] == "1" and ops.conv_gemm is orig_conv and ops.memory_read is orig_mr
 
     # lock-step lane: a cached step object in graph mode must run eagerly for the pass and be restored
-    from mivos_b200.lockstep import _LockStep
+    from mivos_b200.frame_step import FrameStep
+    monkeypatch.setenv("MIVOS_GRAPH", "0")  # read by the cores: they run the step eagerly
     cores = [mv.InferenceCore(net, None, im, bench.K_OBJ, mem_freq=bench.MEM_FREQ, device="cpu") for im in images]
-    monkeypatch.setenv("MIVOS_GRAPH", "0")
     mv.LockstepSession(cores).interact(masks, 0)  # creates and caches the step (eager here: no CUDA graphs on the CPU)
     monkeypatch.setenv("MIVOS_GRAPH", "1")
     steps = list(net.engine().__dict__["_lock_steps"].values())
-    assert len(steps) == 1 and isinstance(steps[0], _LockStep)
+    assert len(steps) == 1 and isinstance(steps[0], FrameStep) and steps[0].C == 2
     steps[0].use_graph = True
     rec2, _ = bench._bracketed_pass(mv, ops, net, images, masks, "cpu")
     assert steps[0].use_graph is True and os.environ["MIVOS_GRAPH"] == "1"

@@ -90,9 +90,9 @@ def test_fusion_host_graph(fuse_sd, golden, monkeypatch):
     _close(ops.halo_to_nchw(lg, 1, H, W, 1), g["fuse"])
 
 
-def test_lockstep_multi_clip_host_graph(eng, golden):
-    """segment_multi / encode_memory_multi (C clips advanced as one batch of C*K maps, per-clip memory
-    read / skip broadcast / stem gather / aggregation on slices) equal the per-clip calls."""
+def test_segment_and_memorize_of_c_clips_equal_per_clip_calls(eng, golden):
+    """segment / encode_memory at C = 3 (C clips advanced as one batch of C*K maps, per-clip memory read / skip
+    broadcast / stem gather / aggregation as groups) equal the same methods at C = 1 per clip."""
     g = golden("ops_lowres.npz")
     keys, values = torch.from_numpy(g["keys"]), torch.from_numpy(g["values"])
     K, _, T, h, w = keys.shape
@@ -106,14 +106,14 @@ def test_lockstep_multi_clip_host_graph(eng, golden):
         ops.bank_from_nchw(kc, vc, bank_k[c * K:(c + 1) * K], bank_v[c * K:(c + 1) * K])
     states, batch = eng.new_query_states(96, 128, C)
     eng.encode_query_batch(frames, batch)
-    prob_multi = eng.segment_multi(bank_k, bank_v, slots, batch, K, C, torch.zeros((C, K + 1, 1, 96, 128)))
+    _, prob_multi = eng.segment(bank_k, bank_v, slots, batch, K, C, prob_out=torch.zeros((C, K + 1, 1, 96, 128)))
     for c in range(C):
         _, prob = eng.segment(bank_k[c * K:(c + 1) * K], bank_v[c * K:(c + 1) * K], slots, states[c], K)
         assert float((prob_multi[c] - prob).abs().max()) <= 1e-5, c
     assert float((prob_multi[0] - torch.from_numpy(g["agg"])).abs().max()) <= 3e-2  # clip 0 is the golden case
     # memorize: clip c's masks are its own probabilities
     masks = prob_multi[:, 1:].contiguous()
-    kv_multi = eng.encode_memory_multi(frames, masks).clone()
+    kv_multi = eng.encode_memory(frames, masks).clone()
     for c in range(C):
         kv = eng.encode_memory(frames[c:c + 1], masks[c])
         assert float((kv_multi[c * K:(c + 1) * K] - kv).abs().max()) <= 1e-4, c

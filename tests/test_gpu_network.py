@@ -125,8 +125,9 @@ def test_three_objects_against_oracle(dev, nets, prop_sd):
 
 def test_graph_replay_is_bit_identical_to_eager(dev, nets):
     """The captured per-frame CUDA graph (device-side bank counters, fixed launch geometry) must
-    reproduce the eager launch sequence bit for bit: the memory read's final selection is exact and
-    totally ordered, so a different split of the memory axis cannot change the result."""
+    reproduce the step's eager launches bit for bit.  That a capacity-sized bank read through the device-side
+    slot count gives what a read of the live slots with a host count gives is checked per read in
+    test_gpu_memread.py, test_gpu_memread_dense.py and test_gpu_memread_wide.py."""
     images, mask = Wt.synthetic_clip(9, 64, 96, 2, seed=11)
     res = []
     for use_graph in (False, True, True):  # second graph run exercises the cached graphs

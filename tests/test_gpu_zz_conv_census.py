@@ -6,7 +6,7 @@ Scenarios (seeded weights and clips of oracle.weights), on fp16 and TF32 unless 
   core480    InferenceCore, 480x864, K = 2, top-k 20, 10 frames (a full query chunk of 8), interactions at frames 0
              and 5 (the second pass fuses): query chunk N = 8, memorize n = 2, segment, decoder split-K with a
              residual, FusionNet (TF32)
-  lock480    LockstepSession of 4 clips x K = 1 at 480x864: encode_memory_multi / segment_multi at n = 4
+  lock480    LockstepSession of 4 clips x K = 1 at 480x864: encode_memory / segment at C = 4, n = 4
   core112    InferenceCore, 112x176, K = 3: 7x11 maps at 1/16, one partial M tile spanning images
   core1080   InferenceCore, 1088x1920 (a 1080p clip), K = 2, 3 frames, a fused second interaction: S = 3 plans
   s2m        the S2M network at 480x864, n = 2, and at 1088x1920, n = 1: im2col stem, dilated K = 18432 under

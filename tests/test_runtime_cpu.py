@@ -92,6 +92,77 @@ def test_lockstep_session_equals_single_clip_passes(rt):
         assert cores[i].certain_mem_k.shape[2] == 2
 
 
+def test_lockstep_session_of_one_clip_equals_interact(rt):
+    """LockstepSession([core]) runs the single-clip step and pass loop: the same bits as core.interact, including a
+    fused second interaction."""
+    from oracle import weights as Wt
+    mv, net, fuse = rt
+    images, mask = Wt.synthetic_clip(7, 64, 96, 2, seed=44)
+    solo = mv.InferenceCore(net, fuse, images, 2, mem_freq=2, device="cpu")
+    core = mv.InferenceCore(net, fuse, images, 2, mem_freq=2, device="cpu")
+    sess = mv.LockstepSession([core])
+    for m, idx in ((mask, 2), (mask.flip(-1).contiguous(), 6)):
+        want = solo.interact(m, idx)
+        (got,) = sess.interact([m], idx)
+        assert torch.equal(core.prob, solo.prob) and np.array_equal(got, want) and np.array_equal(core.np_masks, want)
+        assert core.bank_trace == solo.bank_trace
+    assert "_lock_steps" not in net.engine().__dict__  # one clip shares the single-clip steps
+
+
+def test_frame_step_issues_the_same_operators_for_one_and_three_clips(rt, monkeypatch):
+    """The step of C lock-step clips makes the launch sequence of one clip: the per-clip operators (memory read, skip
+    broadcast, stem gather, aggregation, bank write) take the C clips as groups of one launch each."""
+    import abi_emulator as E
+    from mivos_b200 import ops
+    from mivos_b200.frame_step import FrameStep
+    mv, net, _ = rt
+    names = []
+    for name in E.OPS:
+        monkeypatch.setattr(ops, name, lambda *a, _n=name, _f=getattr(ops, name), **k: (names.append(_n), _f(*a, **k))[1])
+    K, H, W = 2, 64, 96
+    eng = net.engine()
+    seqs = {}
+    for C in (1, 3):
+        step = FrameStep(net, C, K, H, W, 16)
+        step.bank_k.normal_()
+        step.bank_v.normal_()
+        states, batch = eng.new_query_states(H, W, C)
+        eng.encode_query_batch(torch.randn((C, 3, H, W)), batch)
+        frames = [torch.randn((1, 3, H, W)) for _ in range(C)]
+        for memorize in (False, True):
+            step.run(frames, states, 2, 2, memorize, graph=False)  # allocates the workspaces
+            names.clear()
+            step.run(frames, states, 2, 2, memorize, graph=False)
+            seqs[C, memorize] = list(names)
+    for memorize in (False, True):
+        assert seqs[1, memorize] == seqs[3, memorize], memorize
+        assert seqs[1, memorize].count("memory_read") == 1
+    assert seqs[1, True].count("bank_write") == 1 and seqs[1, True].count("stem_gather") == 1
+
+
+def test_a_dropped_network_releases_its_cached_steps(rt, prop_sd):
+    """The frame steps cached on a network's engine do not keep the network alive: dropping it releases its
+    workspaces, banks and graphs at once, not whenever the garbage collector next runs."""
+    import gc
+    import weakref
+    from oracle import weights as Wt
+    mv = rt[0]
+    images, mask = Wt.synthetic_clip(4, 64, 96, 1, seed=3)
+    gc.disable()
+    try:
+        net = mv.PropagationNetwork(top_k=20, act_dtype=torch.float32)
+        net.load_state_dict(prop_sd, strict=True)
+        cores = [mv.InferenceCore(net, None, images, 1, mem_freq=2, device="cpu") for _ in range(3)]
+        cores[0].interact(mask, 1)
+        mv.LockstepSession(cores[1:]).interact([mask, mask], 1)
+        eng = weakref.ref(net.engine())
+        assert eng().__dict__["_frame_steps"] and eng().__dict__["_lock_steps"]
+        del net, cores
+        assert eng() is None
+    finally:
+        gc.enable()
+
+
 def test_lockstep_rejects_clips_that_cannot_share_a_plan(rt):
     from oracle import weights as Wt
     mv, net, _ = rt

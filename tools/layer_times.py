@@ -42,7 +42,7 @@ def wrap(n):
 
 def frame_step(qs):
     qs = net.encode_query_resident(frame, qs)
-    _, prob = net.segment_resident(bank_k, bank_v, T * hw, qs, K)
+    _, prob = net.engine().segment(bank_k, bank_v, T * hw, qs, K)
     net.memorize_resident(frame, prob[1:], bank_k, bank_v, T)
     return qs
 

@@ -1,5 +1,5 @@
 """Per-launch GPU time table of the unit the headline bench times: one lock-step step of C clips
-(segment_multi + encode_memory_multi + bank writes, cfg-2 shapes, 20-frame bank) plus the batched
+(segment + encode_memory at C clips + bank writes, cfg-2 shapes, 20-frame bank) plus the batched
 query pass of 8 frames, eager launches bracketed by CUDA events, reported per CLIP-FRAME.
 usage: python tools/lockstep_layer_times.py [C=4] [fp16|tf32]"""
 import sys, os, collections
@@ -59,9 +59,9 @@ def query_pass():
 
 def step():
     phase[0] = "S"
-    eng.segment_multi(bank_k, bank_v, T * hw, qbatch, K, C, prob)
+    eng.segment(bank_k, bank_v, T * hw, qbatch, K, C, prob_out=prob)
     phase[0] = "M"
-    kv = eng.encode_memory_multi(frames, prob[:, 1:])
+    kv = eng.encode_memory(frames, prob[:, 1:])
     for c in range(C):
         o = slice(c * K, (c + 1) * K)
         ops.bank_write(kv[o], K, H // 16, W // 16, 0, 128, bank_k[o], bank_v[o], T)

@@ -20,7 +20,7 @@ qs = None
 for i in range(reps):
     torch.cuda.nvtx.range_push("frame")
     qs = net.encode_query_resident(frame, qs)
-    _, prob = net.segment_resident(bank_k, bank_v, T * hw, qs, K)
+    _, prob = net.engine().segment(bank_k, bank_v, T * hw, qs, K)
     net.memorize_resident(frame, prob[1:], bank_k, bank_v, T)
     torch.cuda.nvtx.range_pop()
 torch.cuda.synchronize()

@@ -5,7 +5,8 @@ import sys, os, time, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import mivos_b200
-from mivos_b200 import synth, inference_core as IC
+from mivos_b200 import synth
+from mivos_b200.frame_step import FrameStep
 
 torch.set_grad_enabled(False)
 dev = torch.device("cuda:0")
@@ -24,7 +25,7 @@ def one(instrument):
     cpu = collections.defaultdict(float)
     ev = {"step": [], "chunk": []}
     if instrument:
-        orig_run, orig_get, orig_issue = IC._FrameStep.run, core.get_query_kv_buffered, core._issue_query_chunk
+        orig_run, orig_get, orig_issue = FrameStep.run, core.get_query_kv_buffered, core._issue_query_chunk
 
         def run(self, *a, **k):
             t0 = time.perf_counter()
@@ -53,7 +54,7 @@ def one(instrument):
             cpu["issue_chunk"] += time.perf_counter() - t0
             return r
 
-        IC._FrameStep.run = run
+        FrameStep.run = run
         core.get_query_kv_buffered = get
         core._issue_query_chunk = issue
     torch.cuda.synchronize()
@@ -66,7 +67,7 @@ def one(instrument):
     torch.cuda.synchronize()
     wall = time.perf_counter() - t0
     if instrument:
-        IC._FrameStep.run = orig_run
+        FrameStep.run = orig_run
     return wall, t_issue, a.elapsed_time(b), cpu, ev
 
 
