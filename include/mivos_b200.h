@@ -134,6 +134,16 @@ MIVOS_API int mivos_conv_plan(const mivos_conv_args* a, int sms, int* bn, int* s
  * Results do not depend on the tile width, bit for bit (tests/test_gpu_conv_plans.py); another split-K
  * factor is another fp32 summation order.                                                             */
 MIVOS_API int mivos_conv_tile_override(int bn, int splits);
+/* CTAs per SM (1 or 2) mivos_conv_gemm would run `a`'s plan with on a device with `sms` SMs (0: the
+ * current device).  Two CTAs per SM take tiles of up to 64 columns: each one's fill and epilogue run
+ * under the other's main loop.  The residency never changes the tile width or split-K factor, nor any
+ * result bit.  Pure host arithmetic, like mivos_conv_plan.                                             */
+MIVOS_API int mivos_conv_plan_residency(const mivos_conv_args* a, int sms, int* ctas);
+/* Tuning hook: force the residency of the following mivos_conv_gemm calls (process-wide;
+ * mivos_conv_plan_residency reports it).  0: automatic, 1 or 2 CTAs per SM.  2 is rejected while a
+ * tile override forces a tile wider than 64 columns (and such a tile override while 2 is forced); a
+ * call whose automatic tile is wider than 64 columns fails under 2.                                     */
+MIVOS_API int mivos_conv_residency_override(int ctas);
 
 /* Gather kernels that feed mivos_conv_gemm ---------------------------------------------------
  * Every HALO-map operator below takes an element-type flag (`f16`, `out_f16`, `src_f16` ...):

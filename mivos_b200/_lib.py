@@ -70,6 +70,8 @@ SIGNATURES = {
     "mivos_conv_gemm": (_i, [C.POINTER(ConvArgs), _p]),
     "mivos_conv_tile_override": (_i, [_i, _i]),
     "mivos_conv_plan": (_i, [C.POINTER(ConvArgs), _i, C.POINTER(_i), C.POINTER(_i)]),
+    "mivos_conv_plan_residency": (_i, [C.POINTER(ConvArgs), _i, C.POINTER(_i)]),
+    "mivos_conv_residency_override": (_i, [_i]),
     "mivos_stem_gather": (_i, [_p, _p, _i, _i, _i, _p, _i, _i, _i, _l, _l, _p]),
     "mivos_stem_gather_s2d": (_i, [_p, _p, _i, _i, _i, _p, _i, _i, _i, _l, _l, _p]),
     "mivos_gather_s2": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _p]),

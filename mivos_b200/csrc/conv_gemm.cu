@@ -74,19 +74,24 @@ __device__ __forceinline__ float rna_tf32(float x) {
 #include "conv_epilogue.cuh"
 
 constexpr int kConvThreads = 384;  // producer warpgroup + two MMA / epilogue warpgroups
+constexpr int kMaxBnTwoCtas = 64;  // widest tile of the two-CTAs-per-SM class (RegBudget)
 
-// Shared memory: the whole 227 KB a CTA may use.  [0, RING_BYTES) is the stage ring; the mbarriers sit at the top;
-// the epilogue's staging tile [128][BN + 8] (output element type) ends where they begin, so it overlaps only the
-// last stages of the ring, or none.  A prefetched residual (which fills the staging tile) therefore waits only
-// for those stages to drain, and for layers with fewer k-blocks than free stages it waits for nothing.
-template <int BN, int STAGES>
+// Shared memory: the share of the SM's 228 KB each of the CTAS co-resident CTAs may use (the whole 227 KB a
+// CTA may use at CTAS = 1; 113 KB at CTAS = 2, after the 1 KB the driver reserves per CTA).  [0, RING_BYTES) is
+// the stage ring; the mbarriers sit at the top; the epilogue's staging tile [128][BN + 8] (output element type)
+// ends where they begin, so it overlaps only the last stages of the ring, or none.  A prefetched residual (which
+// fills the staging tile) therefore waits only for those stages to drain, and for layers with fewer k-blocks than
+// free stages it waits for nothing.
+template <int BN, int STAGES, int CTAS>
 struct SmemLayout {
+  static_assert(CTAS == 1 || CTAS == 2, "one or two CTAs per SM");
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  static constexpr int TOTAL = 232448 - 1024;  // less the slack for the manual 1024-byte alignment
+  // less the slack for the manual 1024-byte alignment
+  static constexpr int TOTAL = (CTAS == 1 ? 232448 : 233472 / 2 - 1024) - 1024;
   static constexpr int BAR_OFF = TOTAL - 256;  // full[STAGES], empty[STAGES], residual, drain
-  static_assert(RING_BYTES <= BAR_OFF && (2 * STAGES + 2) * 8 <= 256, "stage ring and barriers exceed 227 KB");
+  static_assert(RING_BYTES <= BAR_OFF && (2 * STAGES + 2) * 8 <= 256, "stage ring and barriers exceed the CTA's share");
   // split-K: fp32 partial tile [128][BN + 8] parked over the drained ring; the pad makes the fragment stores
   // (8-byte pieces of 4 rows per half-warp) conflict-free
   static constexpr int ACC_STRIDE = BN + 8;
@@ -101,11 +106,19 @@ struct SmemLayout {
   static_assert(free_stages(4) >= 1, "the fp32 staging tile leaves no ring stage free");
 };
 
-template <int BN, int STAGES, bool F16>
-__global__ void __launch_bounds__(kConvThreads, 1)
+// Register budget per thread of the producer and the MMA warpgroups.  At CTAS = 2 the two CTAs share the register
+// file: 128 * 32 + 256 * 104 = 384 * 80, the cap __launch_bounds__(384, 2) compiles the whole kernel for (the
+// producer spills at 24).  ptxas allocates the consumer path at that cap too, which leaves no room for the
+// wgmma of a 64-accumulator BN = 128 tile: the two-CTA class takes BN 32 and 64.
+template <int CTAS> struct RegBudget { static constexpr uint32_t PRODUCER = 40, CONSUMER = 232; };
+template <> struct RegBudget<2> { static constexpr uint32_t PRODUCER = 32, CONSUMER = 104; };
+
+template <int BN, int STAGES, bool F16, int CTAS>
+__global__ void __launch_bounds__(kConvThreads, CTAS)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const ConvParams p, const int m_tiles) {
-  using L = SmemLayout<BN, STAGES>;
+  static_assert(CTAS == 1 || BN <= kMaxBnTwoCtas, "a BN > 64 tile needs the register file of a whole SM");
+  using L = SmemLayout<BN, STAGES, CTAS>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem base is only guaranteed 16B aligned; round up to the 1024B the swizzle needs
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -155,7 +168,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   pdl_wait();
 
   if (warp < 4) {
-    sm90::setmaxnreg_dec<40>();
+    sm90::setmaxnreg_dec<RegBudget<CTAS>::PRODUCER>();
     if (warp == 1 && res_here) {
       // residual prefetch: once no k-block uses the ring stages under the staging tile any more, bulk-load the rows
       if (drain_it > 0) sm90::mbar_wait_backoff(drain_bar, 0, p.err, 103, 64);
@@ -181,7 +194,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     return;
   }
 
-  sm90::setmaxnreg_inc<232>();
+  sm90::setmaxnreg_inc<RegBudget<CTAS>::CONSUMER>();
   const int wg = warp / 4 - 1;  // 0: rows 0-63, 1: rows 64-127
   const int tw = threadIdx.x - 128 * (wg + 1);
   float acc[BN / 2];
@@ -298,15 +311,21 @@ __global__ void splitk_epilogue_kernel(const ConvParams p, const int bn) {
   }
 }
 
-template <int BN, int STAGES, bool F16>
+template <int BN, int STAGES, bool F16, int CTAS>
 int launch(const mivos_conv_args* a, const ConvParams& p, cudaStream_t stream) {
-  using L = SmemLayout<BN, STAGES>;
+  using L = SmemLayout<BN, STAGES, CTAS>;
   constexpr int smem_bytes = L::TOTAL + 1024;  // slack for the manual 1024B alignment
   static_assert(smem_bytes <= 232448, "shared memory exceeds the 227 KB a CTA may use");
-  auto kernel = conv_gemm_kernel<BN, STAGES, F16>;
+  auto kernel = conv_gemm_kernel<BN, STAGES, F16, CTAS>;
   static bool configured = false;
   if (!configured) {
     MIVOS_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    // the planner counts CTAS CTAs per SM: a kernel that does not reach that residency would run the layer at
+    // the other class's speed under this class's plan
+    int resident = 0;
+    MIVOS_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kernel, kConvThreads, smem_bytes));
+    MIVOS_REQUIRE(resident >= CTAS, "conv_gemm: BN %d kernel of the %d-CTA class reaches %d CTAs per SM", BN, CTAS,
+                  resident);
     configured = true;
   }
   CUtensorMap tmA, tmB;
@@ -332,6 +351,8 @@ using namespace mivos;
 namespace mivos {
 // mivos_conv_tile_override: forced tile width (low 16 bits, 0 = automatic) and split-K factor (high bits, 0 or 1 = one pass)
 std::atomic<int> g_tile_override{0};
+// mivos_conv_residency_override: forced CTAs per SM (0 = automatic)
+std::atomic<int> g_residency_override{0};
 }
 
 namespace mivos {
@@ -346,8 +367,14 @@ namespace {
 // Pure host arithmetic on the argument block (no pointer is dereferenced, no device is touched):
 // exported as mivos_conv_plan so the choice can be unit-tested without a GPU.
 constexpr int64_t kSkCounterBytes = 65536;  // reserved head of the split-K workspace
+// Two CTAs per SM: the main loop's extra cost, as a fraction of it, of sharing the SM and of the shallower ring.
+// Fitted to the H100 sweep tools/residency_sweep.txt (tools/tile_sweep.py residency): every value in [0, 0.7] makes
+// the same choice on all 48 layer forms, and it is right on 47 (the exception costs 0.6 us); from 0.8 on, layers
+// that run faster on two CTAs per SM are kept on one.  Below one wave of one CTA per SM two CTAs per SM only lose
+// (ring depth, nothing to overlap), which a penalty > 0 makes the model say.
+constexpr double kResidencyPenalty = 0.35;
 
-int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits_out) {
+int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits_out, int* ctas_out) {
   const int bk = a->in_f16 ? 64 : 32;
   const int64_t rows = static_cast<int64_t>(a->n) * (a->h + 2) * (a->w + 2);
   const int kblocks = a->cin_pad / bk;
@@ -403,20 +430,54 @@ int plan_tiles(const mivos_conv_args* a, const int sms, int* bn_out, int* splits
       splits = forced_splits;
     }
   }
+  int ctas = 1;
+  if (bn <= kMaxBnTwoCtas) {
+    // Residency, for the (BN, splits) chosen above (it never changes them, so neither does any result): two CTAs
+    // per SM give 2 x SMs slots per round, and one CTA's fill and epilogue run under the other's main loop, so a
+    // co-resident pair costs about max(main loop, epilogue), plus kResidencyPenalty x the main loop.
+    const double ml = kb_total / splits * (16.0 + bn / 8.0 + 6.0);
+    const double ep = bn * out_kb_per_col;
+    const int64_t ctas_total = mtiles * (a->cout_pad / bn) * splits;
+    const double hi = ml > ep ? ml : ep, lo = ml > ep ? ep : ml;
+    const double cost1 = static_cast<double>((ctas_total + sms - 1) / sms) * hi + lo;
+    const double cost2 = static_cast<double>((ctas_total + 2 * sms - 1) / (2 * sms)) * (hi + kResidencyPenalty * ml) + lo;
+    if (cost2 < cost1) ctas = 2;
+  }
+  const int forced_ctas = g_residency_override.load(std::memory_order_relaxed);
+  if (forced_ctas > 0) {
+    MIVOS_REQUIRE(forced_ctas == 1 || bn <= kMaxBnTwoCtas, "conv_gemm: residency override 2 with a BN %d tile (two "
+                  "CTAs per SM take tiles of up to %d columns)", bn, kMaxBnTwoCtas);
+    ctas = forced_ctas;
+  }
   *bn_out = bn;
   *splits_out = splits;
+  *ctas_out = ctas;
   return MIVOS_OK;
 }
 
 }  // namespace
 }  // namespace mivos
 
-extern "C" MIVOS_API int mivos_conv_plan(const mivos_conv_args* a, int sms, int* bn, int* splits) {
-  MIVOS_REQUIRE(a && bn && splits, "conv_plan: null pointer");
+namespace {
+int checked_plan(const mivos_conv_args* a, int sms, int* bn, int* splits, int* ctas) {
+  MIVOS_REQUIRE(a, "conv_plan: null pointer");
   MIVOS_REQUIRE((a->taps == 1 || a->taps == 4 || a->taps == 9) && a->cin_pad > 0 && a->cin_pad % (a->in_f16 ? 64 : 32) == 0 &&
                     a->cout_pad > 0 && a->cout_pad % 32 == 0 && a->n > 0 && a->h > 0 && a->w > 0,
                 "conv_plan: bad shape");
-  return plan_tiles(a, sms > 0 ? sms : num_sms(), bn, splits);
+  return plan_tiles(a, sms > 0 ? sms : num_sms(), bn, splits, ctas);
+}
+}  // namespace
+
+extern "C" MIVOS_API int mivos_conv_plan(const mivos_conv_args* a, int sms, int* bn, int* splits) {
+  MIVOS_REQUIRE(bn && splits, "conv_plan: null pointer");
+  int ctas = 1;
+  return checked_plan(a, sms, bn, splits, &ctas);
+}
+
+extern "C" MIVOS_API int mivos_conv_plan_residency(const mivos_conv_args* a, int sms, int* ctas) {
+  MIVOS_REQUIRE(ctas, "conv_plan_residency: null pointer");
+  int bn = 0, splits = 0;
+  return checked_plan(a, sms, &bn, &splits, ctas);
 }
 
 extern "C" MIVOS_API int mivos_conv_tile_override(int bn, int splits) {
@@ -424,7 +485,18 @@ extern "C" MIVOS_API int mivos_conv_tile_override(int bn, int splits) {
                 "conv_tile_override: tile width %d is not 0, 32, 64, 128 or 256", bn);
   MIVOS_REQUIRE(splits >= 0 && splits <= 0x7fff, "conv_tile_override: bad split-K factor %d", splits);
   MIVOS_REQUIRE(splits < 2 || bn > 0, "conv_tile_override: a split-K factor (%d) needs a forced tile width", splits);
+  MIVOS_REQUIRE(bn <= mivos::kMaxBnTwoCtas || mivos::g_residency_override.load(std::memory_order_relaxed) != 2,
+                "conv_tile_override: BN %d under a residency override of 2 CTAs per SM", bn);
   mivos::g_tile_override.store(bn | (splits << 16), std::memory_order_relaxed);
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_conv_residency_override(int ctas) {
+  MIVOS_REQUIRE(ctas == 0 || ctas == 1 || ctas == 2, "conv_residency_override: %d is not 0, 1 or 2 CTAs per SM", ctas);
+  const int forced_bn = mivos::g_tile_override.load(std::memory_order_relaxed) & 0xffff;
+  MIVOS_REQUIRE(ctas != 2 || forced_bn <= mivos::kMaxBnTwoCtas,
+                "conv_residency_override: 2 CTAs per SM with a forced BN of %d", forced_bn);
+  mivos::g_residency_override.store(ctas, std::memory_order_relaxed);
   return MIVOS_OK;
 }
 
@@ -467,9 +539,9 @@ extern "C" MIVOS_API int mivos_conv_gemm(const mivos_conv_args* a, mivos_stream_
   p.err = device_error_flag();
   MIVOS_REQUIRE(p.rows < (1ll << 31) - 4096, "conv_gemm: too many rows for int32 TMA coordinates");
 
-  int bn = 32, splits = 1;
+  int bn = 32, splits = 1, ctas = 1;
   {
-    const int rc = plan_tiles(a, num_sms(), &bn, &splits);
+    const int rc = plan_tiles(a, num_sms(), &bn, &splits, &ctas);
     if (rc != MIVOS_OK) return rc;
   }
   p.splits = splits;
@@ -477,12 +549,20 @@ extern "C" MIVOS_API int mivos_conv_gemm(const mivos_conv_args* a, mivos_stream_
   p.sk_ws = reinterpret_cast<float*>(static_cast<uint8_t*>(a->splitk_ws) + kSkCounterBytes);
 
   int rc = MIVOS_OK;
-  switch (bn) {
-    // stage counts: a ring of ~190 KB of 128-byte k-block stages (one CTA per SM)
-    case 256: rc = a->in_f16 ? launch<256, 4, true>(a, p, stream) : launch<256, 4, false>(a, p, stream); break;
-    case 128: rc = a->in_f16 ? launch<128, 6, true>(a, p, stream) : launch<128, 6, false>(a, p, stream); break;
-    case 64:  rc = a->in_f16 ? launch<64, 8, true>(a, p, stream) : launch<64, 8, false>(a, p, stream); break;
-    default:  rc = a->in_f16 ? launch<32, 9, true>(a, p, stream) : launch<32, 9, false>(a, p, stream); break;
+  if (ctas == 1) {
+    switch (bn) {
+      // stage counts: a ring of ~190 KB of 128-byte k-block stages (one CTA per SM)
+      case 256: rc = a->in_f16 ? launch<256, 4, true, 1>(a, p, stream) : launch<256, 4, false, 1>(a, p, stream); break;
+      case 128: rc = a->in_f16 ? launch<128, 6, true, 1>(a, p, stream) : launch<128, 6, false, 1>(a, p, stream); break;
+      case 64:  rc = a->in_f16 ? launch<64, 8, true, 1>(a, p, stream) : launch<64, 8, false, 1>(a, p, stream); break;
+      default:  rc = a->in_f16 ? launch<32, 9, true, 1>(a, p, stream) : launch<32, 9, false, 1>(a, p, stream); break;
+    }
+  } else {
+    switch (bn) {
+      // a ring of ~100 KB per CTA (two CTAs per SM)
+      case 64:  rc = a->in_f16 ? launch<64, 4, true, 2>(a, p, stream) : launch<64, 4, false, 2>(a, p, stream); break;
+      default:  rc = a->in_f16 ? launch<32, 5, true, 2>(a, p, stream) : launch<32, 5, false, 2>(a, p, stream); break;
+    }
   }
   if (rc != MIVOS_OK || p.splits == 1) return rc;
   // split-K second pass: one thread per (row, 4 channels)
