@@ -49,6 +49,10 @@ enum {
                                4: + attention_weights (get_W); batched forms for lock-step clips: query sets
                                   (memory_read q_div), groups (stem_gather, upsample4x_sigmoid_aggregate),
                                   skip_n (upsample2x_add) */
+/* Largest object count of one clip: the u8 label map holds K objects + background.  The memory read takes up to
+ * 256 object banks per call; the aggregation kernels of mivos_upsample4x_sigmoid_aggregate / mivos_aggregate_wbg
+ * hold a pixel's objects in registers and take up to 16; their *_planes forms take any count up to this. */
+#define MIVOS_MAX_OBJECTS 255
 MIVOS_API int mivos_abi_version(void);
 MIVOS_API const char* mivos_last_error(void);
 /* MIVOS_OK iff the current device is compute capability 9.0 (there is no other code path). */
@@ -170,6 +174,11 @@ MIVOS_API int mivos_stem_gather(const float* frame, const float* masks, int k_ob
 MIVOS_API int mivos_stem_gather_s2d(const float* frame, const float* masks, int k_objects, int h, int w,
                           void* out, int kpad, int out_f16, int groups, int64_t frame_gstride,
                           int64_t mask_gstride, mivos_stream_t stream);
+/* The K-mask form of mivos_stem_gather_s2d for objects [obj0, obj0 + n_obj) of the K only: out holds n_obj images,
+ * image i being object obj0 + i with its "others" channel summed over ALL K masks except its own, in object order
+ * (prop_net.py:150-157).  Runs a memorize in object chunks with the bits of the whole-clip gather.                */
+MIVOS_API int mivos_stem_gather_s2d_range(const float* frame, const float* masks, int k_objects, int obj0, int n_obj,
+                                int h, int w, void* out, int kpad, int out_f16, mivos_stream_t stream);
 /* Generic strided gather from a HALO map: out[r_out, (ky*ks+kx)*c + ci] for kernel ks (1 or 3),
  * stride 2, pad ks/2 (mod_resnet.py:83-84,140-144 with stride=2).                               */
 MIVOS_API int mivos_gather_s2(const void* in, int n, int h, int w, int c, int in_cstride, int ks,
@@ -279,6 +288,15 @@ MIVOS_API int mivos_upsample4x_sigmoid_aggregate(const float* logits, int k_obje
  * aggregate_sbg (aggregate.py:4-20); keep_bg == 0 drops row 0 from the output.                  */
 MIVOS_API int mivos_aggregate_wbg(const float* prob, int k_objects, int64_t hw, int keep_bg, int hard,
                         float* out, mivos_stream_t stream);
+/* The same two operators for 1 <= K <= MIVOS_MAX_OBJECTS, with no per-thread object arrays: the sigmoid
+ * planes are written first (the object planes of prob_out) and the aggregation makes per-pixel passes over
+ * them — background product, logits and their maximum, exp-sum, normalisation — in the operation order of the
+ * register kernels, whose bits they give for K <= 16.  prob_out may not alias raw_out.                       */
+MIVOS_API int mivos_upsample4x_sigmoid_aggregate_planes(const float* logits, int k_objects, int h4, int w4,
+                                              int cstride, int coff, float* raw_out, float* prob_out, int groups,
+                                              mivos_stream_t stream);
+MIVOS_API int mivos_aggregate_wbg_planes(const float* prob, int k_objects, int64_t hw, int keep_bg, int hard,
+                               float* out, mivos_stream_t stream);
 /* argmax over the K+1 rows of prob [(K+1), T, 1, nh, nw] for frame range, fused with unpad:
  * writes masks_padded [T,1,nh,nw] u8 and (optional) masks_out [T,h,w] u8
  * (inference_core.py:259-269).                                                                  */

@@ -74,6 +74,7 @@ SIGNATURES = {
     "mivos_conv_residency_override": (_i, [_i]),
     "mivos_stem_gather": (_i, [_p, _p, _i, _i, _i, _p, _i, _i, _i, _l, _l, _p]),
     "mivos_stem_gather_s2d": (_i, [_p, _p, _i, _i, _i, _p, _i, _i, _i, _l, _l, _p]),
+    "mivos_stem_gather_s2d_range": (_i, [_p, _p, _i, _i, _i, _i, _i, _p, _i, _i, _p]),
     "mivos_gather_s2": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _p]),
     "mivos_maxpool3x3s2": (_i, [_p, _i, _i, _i, _i, _p, _i, _p]),
     "mivos_upsample2x_add": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _i, _p]),
@@ -92,6 +93,8 @@ SIGNATURES = {
     "mivos_memory_read_wide": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _p, _i, _p]),
     "mivos_upsample4x_sigmoid_aggregate": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p]),
     "mivos_aggregate_wbg": (_i, [_p, _i, _l, _i, _i, _p, _p]),
+    "mivos_upsample4x_sigmoid_aggregate_planes": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _i, _p]),
+    "mivos_aggregate_wbg_planes": (_i, [_p, _i, _l, _i, _i, _p, _p]),
     "mivos_argmax_unpad": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p]),
     "mivos_frames_u8_normalize": (_i, [_p, _i, _i, _i, _p, _p]),
     "mivos_pad2d": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _p, _p]),

@@ -7,13 +7,13 @@ from . import ops
 
 
 def aggregate_wbg(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False) -> torch.Tensor:
-    """aggregate.py:22-37: bg = prod(1-p); clamp; logit (x1000 if hard); softmax over K+1."""
-    return ops.aggregate_wbg(prob.detach().float().contiguous(), keep_bg=keep_bg, hard=hard)
+    """aggregate.py:22-37: bg = prod(1-p); clamp; logit (x1000 if hard); softmax over K+1.  1 <= K <= 255."""
+    return ops.aggregate_any(prob.detach().float().contiguous(), keep_bg=keep_bg, hard=hard)
 
 
 def aggregate_sbg(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False) -> torch.Tensor:
-    """aggregate.py:4-20: constant 0.5 background instead of prod(1-p)."""
-    return ops.aggregate_wbg(prob.detach().float().contiguous(), keep_bg=keep_bg, hard=hard, const_bg=True)
+    """aggregate.py:4-20: constant 0.5 background instead of prod(1-p).  1 <= K <= 255."""
+    return ops.aggregate_any(prob.detach().float().contiguous(), keep_bg=keep_bg, hard=hard, const_bg=True)
 
 
 def aggregate_wbg_channel(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False):

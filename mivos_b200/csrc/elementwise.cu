@@ -147,6 +147,89 @@ __global__ void upsample4x_sigmoid_aggregate_kernel(const float* __restrict__ lo
   }
 }
 
+// ---- aggregation over any object count (mivos_*_planes).  The kernels above hold a pixel's K values in
+// per-thread arrays of kMaxObjects; these hold none: the object values live in planes in global memory and a
+// thread makes passes over them — background product, logits (written over the planes) and their maximum,
+// exponentials (written over the logits) and their sum, normalisation — in the operation order of
+// aggregate_pixel, so for K <= 16 they give its bits.
+__device__ __forceinline__ float clamped_logit(float v, bool hard) {
+  v = fminf(fmaxf(v, 1e-7f), 1.f - 1e-7f);
+  float l = logf(v / (1.f - v));
+  if (hard) l *= 1000.f;
+  return l;
+}
+
+// Group g, pixel i: object j at in[g*in_gstride + j*plane + i]; the result at out[g*out_gstride + ...], background
+// first when keep_bg.  `in` may be the object planes of `out` itself (in place: in == out + plane, keep_bg).
+__global__ void aggregate_planes_kernel(const float* in, int kobj, int64_t plane, int groups, int64_t in_gstride,
+                                        float* out, int64_t out_gstride, int keep_bg, int hard) {
+  mivos::pdl_prologue();
+  const bool hl = (hard & 1) != 0;
+  for (int64_t ig = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; ig < plane * groups;
+       ig += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t g = ig / plane, i = ig - g * plane;
+    const float* p = in + g * in_gstride + i;
+    float* o = out + g * out_gstride + i;
+    float* ob = keep_bg ? o + plane : o;  // object j of the result at ob[j * plane]
+    float bg = 1.f;
+    if (hard & 2) {
+      bg = 0.5f;  // aggregate_sbg (aggregate.py:8)
+    } else {
+      for (int j = 0; j < kobj; ++j) bg *= (1.f - p[j * plane]);
+    }
+    const float l0 = clamped_logit(bg, hl);
+    float mx = l0;
+    for (int j = 0; j < kobj; ++j) {
+      const float l = clamped_logit(p[j * plane], hl);
+      ob[j * plane] = l;
+      mx = fmaxf(mx, l);
+    }
+    const float e0 = expf(l0 - mx);
+    float s = e0;
+    for (int j = 0; j < kobj; ++j) {
+      const float e = expf(ob[j * plane] - mx);
+      ob[j * plane] = e;
+      s += e;
+    }
+    if (keep_bg) o[0] = e0 / s;
+    for (int j = 0; j < kobj; ++j) ob[j * plane] = ob[j * plane] / s;
+  }
+}
+
+// x4 bilinear + sigmoid of every object map, one thread per (image, pixel): image g*kobj + j of the logits to
+// raw_all[(g*kobj + j)*plane] and/or obj_all[g*obj_gstride + j*plane] (the object planes of a prob volume).
+__global__ void upsample4x_sigmoid_planes_kernel(const float* __restrict__ logits, int kobj, int h4, int w4,
+                                                 int cstride, int coff, int groups, float* __restrict__ raw_all,
+                                                 float* __restrict__ obj_all, int64_t obj_gstride) {
+  mivos::pdl_prologue();
+  const int H = 4 * h4, W = 4 * w4;
+  const int64_t plane = static_cast<int64_t>(H) * W;
+  const int64_t total = plane * kobj * groups;
+  for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < total;
+       t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t img = t / plane, i = t - img * plane;
+    const int y = static_cast<int>(i / W), x = static_cast<int>(i - static_cast<int64_t>(y) * W);
+    int y0, y1, x0, x1;
+    float ly, lx;
+    bilin(y, 0.25f, h4, y0, y1, ly);
+    bilin(x, 0.25f, w4, x0, x1, lx);
+    const float hy = 1.f - ly, hx = 1.f - lx;
+    const int64_t base = img * (h4 + 2);
+    const float v00 = logits[((base + y0 + 1) * (w4 + 2) + x0 + 1) * cstride + coff];
+    const float v01 = logits[((base + y0 + 1) * (w4 + 2) + x1 + 1) * cstride + coff];
+    const float v10 = logits[((base + y1 + 1) * (w4 + 2) + x0 + 1) * cstride + coff];
+    const float v11 = logits[((base + y1 + 1) * (w4 + 2) + x1 + 1) * cstride + coff];
+    // the roundings the compiler picks for the same expression in upsample4x_sigmoid_aggregate_kernel, spelled out
+    const float v = __fmaf_rn(hy, __fmaf_rn(hx, v00, __fmul_rn(lx, v01)), __fmul_rn(ly, __fmaf_rn(hx, v10, __fmul_rn(lx, v11))));
+    const float p = sigmoidf_exact(v);
+    if (raw_all) raw_all[t] = p;
+    if (obj_all) {
+      const int64_t g = img / kobj, j = img - g * kobj;
+      obj_all[g * obj_gstride + j * plane + i] = p;
+    }
+  }
+}
+
 // bilinear resize (align_corners=False, any ratio) of ONE channel of a HALO map to NCHW planes
 // [n,1,H,W], optionally through a sigmoid: the final F.interpolate of the S2M network
 // (model/s2m/utils.py:20) and the torch.sigmoid its callers apply (davis_processor.py:68,
@@ -461,10 +544,42 @@ extern "C" MIVOS_API int mivos_aggregate_wbg(const float* prob, int k_objects, i
   return MIVOS_OK;
 }
 
+extern "C" MIVOS_API int mivos_upsample4x_sigmoid_aggregate_planes(const float* logits, int k_objects, int h4, int w4,
+                                                                   int cstride, int coff, float* raw_out,
+                                                                   float* prob_out, int groups, mivos_stream_t s) {
+  MIVOS_REQUIRE(logits && (raw_out || prob_out), "upsample4x_planes: null pointer");
+  MIVOS_REQUIRE(k_objects >= 1 && k_objects <= MIVOS_MAX_OBJECTS, "upsample4x_planes: %d objects (1 to %d)", k_objects,
+                MIVOS_MAX_OBJECTS);
+  MIVOS_REQUIRE(groups >= 1 && h4 >= 1 && w4 >= 1 && coff >= 0 && coff < cstride, "upsample4x_planes: bad shape");
+  const int64_t plane = 16ll * h4 * w4;
+  const int64_t pgs = (k_objects + 1) * plane;  // prob volume of one group
+  launch_pdl(upsample4x_sigmoid_planes_kernel, capped_grid(plane * k_objects * groups), kThreads, 0, ST(s), logits,
+             k_objects, h4, w4, cstride, coff, groups, raw_out, prob_out ? prob_out + plane : nullptr, pgs);
+  MIVOS_LAUNCHED();
+  if (prob_out) {  // in place: the object planes written above become the result
+    launch_pdl(aggregate_planes_kernel, capped_grid(plane * groups), kThreads, 0, ST(s),
+               static_cast<const float*>(prob_out + plane), k_objects, plane, groups, pgs, prob_out, pgs, 1, 0);
+    MIVOS_LAUNCHED();
+  }
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_aggregate_wbg_planes(const float* prob, int k_objects, int64_t hw, int keep_bg, int hard,
+                                                    float* out, mivos_stream_t s) {
+  MIVOS_REQUIRE(prob && out, "aggregate_wbg_planes: null pointer");
+  MIVOS_REQUIRE(k_objects >= 1 && k_objects <= MIVOS_MAX_OBJECTS, "aggregate_wbg_planes: %d objects (1 to %d)",
+                k_objects, MIVOS_MAX_OBJECTS);
+  MIVOS_REQUIRE(hw >= 1 && hard >= 0 && hard <= 3, "aggregate_wbg_planes: bad arguments");
+  launch_pdl(aggregate_planes_kernel, capped_grid(hw), kThreads, 0, ST(s), prob, k_objects, hw, 1, int64_t{0}, out,
+             int64_t{0}, keep_bg ? 1 : 0, hard);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
 extern "C" MIVOS_API int mivos_argmax_unpad(const float* prob, int k_plus_1, int t, int nh, int nw,
                                             int pad_l, int pad_t, int h, int w, uint8_t* masks_padded,
                                             uint8_t* masks_out, mivos_stream_t s) {
-  MIVOS_REQUIRE(prob && masks_padded && k_plus_1 >= 1 && k_plus_1 <= 255, "argmax_unpad: bad arguments");
+  MIVOS_REQUIRE(prob && masks_padded && k_plus_1 >= 1 && k_plus_1 <= MIVOS_MAX_OBJECTS + 1, "argmax_unpad: bad arguments");
   const int64_t total = static_cast<int64_t>(t) * nh * nw;
   launch_pdl(argmax_unpad_kernel, capped_grid(total), kThreads, 0, ST(s), prob, k_plus_1, t, nh, nw, pad_l, pad_t,
                                                                   h, w, masks_padded, masks_out);

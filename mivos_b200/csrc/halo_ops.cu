@@ -206,7 +206,8 @@ cudaError_t reserve_stem_smem(int smem) {
 template <int CIN, typename T>
 __global__ void __launch_bounds__(256)
 stem_s2d_gather_kernel(const float* __restrict__ frame, const float* __restrict__ masks, int kobj, int h, int w,
-                       T* __restrict__ out, int kpad, int64_t frame_gstride, int64_t mask_gstride) {
+                       T* __restrict__ out, int kpad, int64_t frame_gstride, int64_t mask_gstride, int obj0,
+                       int nobj) {
   mivos::pdl_prologue();
   extern __shared__ __align__(16) uint8_t s2d_smem[];
   T* rowbuf = reinterpret_cast<T*>(s2d_smem);  // [2][w + 8][CIN]
@@ -214,10 +215,11 @@ stem_s2d_gather_kernel(const float* __restrict__ frame, const float* __restrict_
   const int wp = wo + 2;
   const int yo = static_cast<int>(blockIdx.x) - 1;  // output row; -1 and ho are border rows (zeros)
   const int img = blockIdx.y;
-  const int obj = CIN == 5 ? img % kobj : img;
+  // the mask form gathers objects [obj0, obj0 + nobj) of each group of kobj (all of them but in object-chunked memorize)
+  const int obj = CIN == 5 ? obj0 + img % nobj : img;
   if constexpr (CIN == 5) {
-    frame += static_cast<int64_t>(img / kobj) * frame_gstride;
-    masks += static_cast<int64_t>(img / kobj) * mask_gstride;
+    frame += static_cast<int64_t>(img / nobj) * frame_gstride;
+    masks += static_cast<int64_t>(img / nobj) * mask_gstride;
   }
   const int64_t plane = static_cast<int64_t>(h) * w;
   const int rowlen = (w + 8) * CIN;
@@ -665,18 +667,16 @@ extern "C" MIVOS_API int mivos_stem_gather(const float* frame, const float* mask
   return MIVOS_OK;
 }
 
-extern "C" MIVOS_API int mivos_stem_gather_s2d(const float* frame, const float* masks, int k_objects, int h, int w,
-                                               void* out, int kpad, int out_f16, int groups, int64_t frame_gstride,
-                                               int64_t mask_gstride, mivos_stream_t s) {
-  MIVOS_REQUIRE(frame && out, "stem_gather_s2d: null pointer");
-  MIVOS_REQUIRE(groups >= 1 && (masks || groups == 1), "stem_gather_s2d: groups need the mask form (one frame + K masks per group)");
-  MIVOS_REQUIRE(h % 2 == 0 && w % 2 == 0 && h > 0 && w > 0 && k_objects >= 1, "stem_gather_s2d: h,w must be even");
+namespace {
+// launches stem_s2d_gather_kernel for images [obj0, obj0 + nobj) of each of `groups` groups of k_objects
+int stem_s2d(const char* who, const float* frame, const float* masks, int k_objects, int obj0, int nobj, int h, int w,
+             void* out, int kpad, int out_f16, int groups, int64_t frame_gstride, int64_t mask_gstride, mivos_stream_t s) {
   const int cin = masks ? 5 : 3;
   const int v = out_f16 ? 8 : 4;
-  MIVOS_REQUIRE(kpad >= 16 * cin && kpad % v == 0 && AL16(out), "stem_gather_s2d: kpad %d too small for cin %d / unaligned", kpad, cin);
-  const dim3 grid(h / 2 + 2, k_objects * groups);
+  MIVOS_REQUIRE(kpad >= 16 * cin && kpad % v == 0 && AL16(out), "%s: kpad %d too small for cin %d / unaligned", who, kpad, cin);
+  const dim3 grid(h / 2 + 2, nobj * groups);
   const int smem = 2 * (w + 8) * cin * (out_f16 ? 2 : 4);
-  MIVOS_REQUIRE(smem <= 227 * 1024, "stem_gather_s2d: a %d-pixel wide frame needs %d B of shared memory", w, smem);
+  MIVOS_REQUIRE(smem <= 227 * 1024, "%s: a %d-pixel wide frame needs %d B of shared memory", who, w, smem);
 #define S2D(CIN_, T_)                                                                                      \
   do {                                                                                                     \
     static int configured = 48 * 1024;                                                                     \
@@ -685,7 +685,7 @@ extern "C" MIVOS_API int mivos_stem_gather_s2d(const float* frame, const float* 
       configured = smem;                                                                                   \
     }                                                                                                      \
     launch_pdl(stem_s2d_gather_kernel<CIN_, T_>, grid, 256, smem, ST(s), frame, masks, k_objects, h, w,    \
-               static_cast<T_*>(out), kpad, frame_gstride, mask_gstride);                                  \
+               static_cast<T_*>(out), kpad, frame_gstride, mask_gstride, obj0, nobj);                      \
   } while (0)
   if (out_f16) {
     if (masks) S2D(5, __half);
@@ -697,6 +697,27 @@ extern "C" MIVOS_API int mivos_stem_gather_s2d(const float* frame, const float* 
 #undef S2D
   MIVOS_LAUNCHED();
   return MIVOS_OK;
+}
+}  // namespace
+
+extern "C" MIVOS_API int mivos_stem_gather_s2d(const float* frame, const float* masks, int k_objects, int h, int w,
+                                               void* out, int kpad, int out_f16, int groups, int64_t frame_gstride,
+                                               int64_t mask_gstride, mivos_stream_t s) {
+  MIVOS_REQUIRE(frame && out, "stem_gather_s2d: null pointer");
+  MIVOS_REQUIRE(groups >= 1 && (masks || groups == 1), "stem_gather_s2d: groups need the mask form (one frame + K masks per group)");
+  MIVOS_REQUIRE(h % 2 == 0 && w % 2 == 0 && h > 0 && w > 0 && k_objects >= 1, "stem_gather_s2d: h,w must be even");
+  return stem_s2d("stem_gather_s2d", frame, masks, k_objects, 0, k_objects, h, w, out, kpad, out_f16, groups,
+                  frame_gstride, mask_gstride, s);
+}
+
+extern "C" MIVOS_API int mivos_stem_gather_s2d_range(const float* frame, const float* masks, int k_objects, int obj0,
+                                                     int n_obj, int h, int w, void* out, int kpad, int out_f16,
+                                                     mivos_stream_t s) {
+  MIVOS_REQUIRE(frame && masks && out, "stem_gather_s2d_range: null pointer");
+  MIVOS_REQUIRE(h % 2 == 0 && w % 2 == 0 && h > 0 && w > 0, "stem_gather_s2d_range: h,w must be even");
+  MIVOS_REQUIRE(k_objects >= 1 && obj0 >= 0 && n_obj >= 1 && obj0 + n_obj <= k_objects && n_obj <= 65535,
+                "stem_gather_s2d_range: objects [%d, %d + %d) outside [0, %d)", obj0, obj0, n_obj, k_objects);
+  return stem_s2d("stem_gather_s2d_range", frame, masks, k_objects, obj0, n_obj, h, w, out, kpad, out_f16, 1, 0, 0, s);
 }
 
 extern "C" MIVOS_API int mivos_stem_gather_frames(const float* frames, int n, int cin, int h, int w, void* out,

@@ -23,6 +23,23 @@ from ._lib import MivosError
 from .ops import PackedConv
 
 BN_EPS = 1e-5
+CHUNK_OBJECTS = 16  # most object maps one memorize / decoder batch takes
+
+
+def object_chunks(K: int):
+    """(first object, count) of the object chunks a clip of K objects runs its memorize and decoder in: one chunk up
+    to CHUNK_OBJECTS, else ceil(K / CHUNK_OBJECTS) chunks of near-equal size (the larger ones first), so that every
+    convolution keeps a batch shape of at most CHUNK_OBJECTS maps and its workspace stays at that size."""
+    if K <= CHUNK_OBJECTS:
+        return [(0, K)]
+    m = -(-K // CHUNK_OBJECTS)
+    q, r = divmod(K, m)
+    chunks, k0 = [], 0
+    for i in range(m):
+        n = q + (1 if i < r else 0)
+        chunks.append((k0, n))
+        k0 += n
+    return chunks
 
 
 class Workspace:
@@ -323,21 +340,36 @@ class PropagationEngine(_ResNetTrunk):
         self.encode_query_batch(frame.reshape(1, 3, H, W), qs)
         return qs
 
-    def encode_memory(self, frames: torch.Tensor, masks: torch.Tensor) -> torch.Tensor:
+    def encode_memory(self, frames: torch.Tensor, masks: torch.Tensor, objs: Optional[Tuple[int, int]] = None) -> torch.Tensor:
         """memorize (prop_net.py:144-162) of one clip (frame [1,3,H,W], masks [K,1,H,W]) or of C clips (frames
         [C,3,H,W], masks [C,K,1,H,W], any clip stride): returns the HALO [C*K,H/16,W/16,640] key|value map, clip-major
         (a workspace buffer: consume before the next call).  The "others" channel sums over the objects of the SAME
-        clip: the stem gather takes the C (frame, K masks) groups in one launch."""
+        clip: the stem gather takes the C (frame, K masks) groups in one launch.  `objs` (k0, n), one clip only:
+        objects [k0, k0 + n) alone ([n,...] map), their "others" channels still summed over all K masks."""
         H, W = masks.shape[-2:]
         N = masks.shape[:-3].numel()  # K, or C*K
         pcs = self.pc["mask_rgb_encoder.conv1"]
-        stem = self.ws.mat("stem_m", N * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
-        ops.stem_gather(frames.reshape(-1, 3, H, W), masks, stem, s2d=True)
+        if objs is None or objs == (0, N):
+            stem = self.ws.mat("stem_m", N * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
+            ops.stem_gather(frames.reshape(-1, 3, H, W), masks, stem, s2d=True)
+        else:
+            k0, N = objs
+            stem = self.ws.mat("stem_m", N * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
+            ops.stem_gather_range(frames, masks, k0, N, stem)
         f16 = self._trunk("mask_rgb_encoder", arch.MASK_LAYERS, stem, N, H, W, {}, self.ws)
         h16, w16 = H // 16, W // 16
         kv = self.ws.halo("kv_m", N, h16, w16, 640, torch.float32)
         _cg(self.ws, f16, self.pc["kv_m_f16"], N, h16, w16, kv)
         return kv
+
+    def memorize_into(self, frames: torch.Tensor, masks: torch.Tensor, bank_k, bank_v, t: int, dyn_t=None) -> None:
+        """encode_memory + bank_write into bank frame `t` (or the device scalar dyn_t, t its largest value) for every
+        object: C clips of K <= CHUNK_OBJECTS objects in one batch, one clip of more objects in object_chunks."""
+        H, W = masks.shape[-2:]
+        N = masks.shape[:-3].numel()
+        for k0, n in ([(0, N)] if masks.dim() == 5 else object_chunks(N)):
+            kv = self.encode_memory(frames, masks, (k0, n))
+            ops.bank_write(kv, n, H // 16, W // 16, 0, 128, bank_k[k0:k0 + n], bank_v[k0:k0 + n], t, dyn_t=dyn_t)
 
     # ------------------------------------------------------------------ decoder
     def _resblock(self, p, x_raw, x_relu, n, h, w, cin, cout, out, *, out_relu_only=False, out_relu=None, ws=None):
@@ -386,9 +418,25 @@ class PropagationEngine(_ResNetTrunk):
         clips.  The C*K object maps (clip-major: map c*K + k is object k of clip c) go through every convolution as
         ONE batch — the 1/16- and 1/8-resolution layers of a single clip have 14-54 row tiles for 132 SMs — while the
         operators whose operands differ per clip (memory read, skip broadcast, aggregation) take the C clips as groups
-        of one launch.  bank_k/bank_v [C*K, cap, 128/512]; `q` the QueryState of one clip's frame, or for C > 1 the
-        batched state of the C current frames (new_query_states(H, W, C)).  Returns (raw sigmoid [C*K,1,H,W] | None,
-        prob [(K+1),1,H,W] | None), prob [C,K+1,1,H,W] for C > 1."""
+        of one launch.  One clip of more than CHUNK_OBJECTS objects runs the read and the decoder per object chunk
+        (object_chunks), each chunk writing its slice of one K-object logits map; one aggregation over all K follows.
+        bank_k/bank_v [C*K, cap, 128/512]; `q` the QueryState of one clip's frame, or for C > 1 the batched state of
+        the C current frames (new_query_states(H, W, C)).  Returns (raw sigmoid [C*K,1,H,W] | None, prob
+        [(K+1),1,H,W] | None), prob [C,K+1,1,H,W] for C > 1."""
+        H, W = q.h, q.w
+        chunks = object_chunks(K) if C == 1 else [(0, K)]
+        if len(chunks) == 1:
+            lg = self._decode(bank_k, bank_v, slots, q, K, C, dyn_slots, None)
+        else:
+            lg = self.ws.halo("logit", K, H // 4, W // 4, 32, torch.float32)
+            for k0, n in chunks:
+                self._decode(bank_k[k0:k0 + n], bank_v[k0:k0 + n], slots, q, n, 1, dyn_slots, lg[k0:k0 + n])
+        return ops.upsample4x_sigmoid_aggregate_any(lg, K, H // 4, W // 4, want_raw=want_raw, want_prob=want_prob,
+                                                    prob_out=prob_out, groups=C)
+
+    def _decode(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int, dyn_slots, lg):
+        """Memory read and decoder of C*K object maps as one batch; returns their decoder.pred logits in `lg` (a
+        workspace map when None)."""
         ws, pc = self.ws, self.pc
         H, W = q.h, q.w
         h16, w16 = H // 16, W // 16
@@ -407,10 +455,10 @@ class PropagationEngine(_ResNetTrunk):
         self._upblock_tail("decoder.up_16_8", q.s8, x16, N, H // 8, W // 8, 512, 256, x8, final_relu=False)
         x4 = ws.halo("dec4", N, H // 4, W // 4, 256)
         self._upblock_tail("decoder.up_8_4", q.s4, x8, N, H // 4, W // 4, 256, 256, x4, final_relu=True)
-        lg = ws.halo("logit", N, H // 4, W // 4, 32, torch.float32)
+        if lg is None:
+            lg = ws.halo("logit", N, H // 4, W // 4, 32, torch.float32)
         _cg(ws, x4, pc["decoder.pred"], N, H // 4, W // 4, lg)
-        return ops.upsample4x_sigmoid_aggregate(lg, K, H // 4, W // 4, want_raw=want_raw, want_prob=want_prob,
-                                                prob_out=prob_out, groups=C)
+        return lg
 
     def _upblock_tail(self, p, s2_skip, up, K, h, w, up_c, out_c, out, final_relu):
         """x = skip (one map per frame, broadcast over that frame's objects) + bilinear_x2(up); out_conv ResBlock."""

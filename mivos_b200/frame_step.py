@@ -85,10 +85,9 @@ class FrameStep:
             eng.segment(self.bank_k, self.bank_v, self.cap_frames * self.hw, self.q, K, C, prob_out=self.out,
                         dyn_slots=self.dyn[0:1])
             if memorize:
-                kv = eng.encode_memory(self.frames, self.masks)
-                # the C*K object banks are contiguous and share the frame slot: one launch
-                ops.bank_write(kv, C * K, self.nh // 16, self.nw // 16, 0, 128, self.bank_k, self.bank_v,
-                               self.cap_frames - 1, dyn_t=self.dyn[1:2])
+                # the C*K object banks are contiguous and share the frame slot: one bank write per object chunk
+                eng.memorize_into(self.frames, self.masks, self.bank_k, self.bank_v, self.cap_frames - 1,
+                                  dyn_t=self.dyn[1:2])
             ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, C * (K + 1), False, self.plane_bytes)
 
     def run(self, frames: Sequence[Optional[torch.Tensor]], cached, visible: int, m_front: int, memorize: bool,

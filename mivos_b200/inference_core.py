@@ -25,7 +25,7 @@ import torch
 import os
 
 from . import _lib, ops, schedule
-from .engine import QueryState
+from .engine import QueryState, object_chunks
 from .frame_step import FrameStep
 from .tensor_util import pad_divide_by
 
@@ -55,6 +55,7 @@ class InferenceCore:
 
         t = images.shape[1]
         h, w = images.shape[-2:]
+        ops.check_objects(num_objects, "InferenceCore")
         self.k = num_objects
         images = images.float()
         self.images, self.pad = pad_divide_by(images, 16, images.shape[-2:])  # :71
@@ -263,7 +264,7 @@ class InferenceCore:
                 attn = self.prop_net.get_attention(mk16[k - 1:k], self.pos_mask_diff[k:k + 1], self.neg_mask_diff[k:k + 1], qk16)
             self.fuse_net.forward_sigmoid_plane(im, prev_mask[k:k + 1].contiguous(), curr_mask[k:k + 1].contiguous(), attn,
                                                 nc, nr, prob[k - 1, 0])
-        return ops.aggregate_wbg(prob, keep_bg=True)
+        return ops.aggregate_any(prob, keep_bg=True)
 
     # ------------------------------------------------------------------ interaction (:219-271)
     def interact(self, mask, idx, total_cb=None, step_cb=None):
@@ -278,7 +279,10 @@ class InferenceCore:
     def _passes_can_overlap(self, idx) -> bool:
         """Both passes non-empty, graph replay on, the clip resident on the device (the host-clip staging slots
         of mem_profile >= 1 are recycled in issue order), and no pass bounded by another interaction (the fusion
-        path shares FusionNet's workspace).  MIVOS_BIDIR=0 forces the sequential order."""
+        path shares FusionNet's workspace), and no more objects than one chunk (object_chunks): a second lane would
+        hold a second bank, 34 GB at 255 objects over 101 480p frames.  MIVOS_BIDIR=0 forces the sequential order."""
+        if len(object_chunks(self.k)) > 1:
+            return False
         if not self.overlap_passes or not self.use_graph or self.data_dev != self.device:
             return False
         if not (0 < idx < self.t - 1):

@@ -26,6 +26,7 @@ import numpy as np
 import torch
 
 from ._lib import MivosError
+from .engine import CHUNK_OBJECTS
 from .inference_core import InferenceCore, run_pass
 
 
@@ -34,6 +35,9 @@ class LockstepSession:
         if len(cores) < 1:
             raise MivosError("LockstepSession needs at least one InferenceCore")
         c0 = cores[0]
+        if c0.k > CHUNK_OBJECTS:
+            raise MivosError(f"LockstepSession: {c0.k} objects per clip; lock-step clips take at most {CHUNK_OBJECTS} "
+                             "(more objects run in object chunks, which only InferenceCore does): run the clips separately")
         for c in cores[1:]:
             same = (c.prop_net is c0.prop_net and c.device == c0.device and c.k == c0.k and c.t == c0.t and c.nh == c0.nh
                     and c.nw == c0.nw and c.mem_freq == c0.mem_freq and c.interacted == c0.interacted)

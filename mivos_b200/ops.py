@@ -258,6 +258,16 @@ def stem_gather(frame: torch.Tensor, masks: Optional[torch.Tensor], out: torch.T
     return out
 
 
+def stem_gather_range(frame: torch.Tensor, masks: torch.Tensor, obj0: int, n: int, out: torch.Tensor) -> torch.Tensor:
+    """The space-to-depth memorize stem (stem_gather with s2d=True) of objects [obj0, obj0 + n) of the K masks
+    [K,1,H,W] only: n output images whose "others" channel still sums over all K objects."""
+    _req(frame), _req(masks), _req_act(out)
+    h, w = frame.shape[-2:]
+    check(_lib.lib().mivos_stem_gather_s2d_range(_ptr(frame), _ptr(masks), masks.shape[0], obj0, n, h, w, _ptr(out),
+                                                 out.shape[-1], _f16(out), _stream()), "mivos_stem_gather_s2d_range")
+    return out
+
+
 def gather_s2(x: torch.Tensor, n: int, h: int, w: int, c: int, ks: int, out: torch.Tensor) -> torch.Tensor:
     _req_act(x), _req_act(out)
     check(_lib.lib().mivos_gather_s2(_ptr(x), n, h, w, c, x.shape[-1], ks, _ptr(out), out.shape[-1],
@@ -460,6 +470,27 @@ def upsample4x_sigmoid_aggregate(logits: torch.Tensor, k: int, h4: int, w4: int,
     return raw, prob
 
 
+def upsample4x_sigmoid_aggregate_planes(logits: torch.Tensor, k: int, h4: int, w4: int, coff: int = 0,
+                                        want_raw: bool = False, want_prob: bool = True,
+                                        raw_out: Optional[torch.Tensor] = None, prob_out: Optional[torch.Tensor] = None,
+                                        groups: int = 1):
+    """upsample4x_sigmoid_aggregate for 1 <= k <= MAX_OBJECTS (mivos_upsample4x_sigmoid_aggregate_planes): no
+    per-thread object arrays, the same bits for k <= 16."""
+    _req(logits)
+    dev = logits.device
+    lead = (groups,) if groups > 1 else ()
+    raw = raw_out if raw_out is not None else (
+        torch.empty((groups * k, 1, 4 * h4, 4 * w4), dtype=torch.float32, device=dev) if want_raw else None)
+    prob = prob_out if prob_out is not None else (
+        torch.empty(lead + (k + 1, 1, 4 * h4, 4 * w4), dtype=torch.float32, device=dev) if want_prob else None)
+    if prob is not None:
+        _req(prob)
+    check(_lib.lib().mivos_upsample4x_sigmoid_aggregate_planes(_ptr(logits), k, h4, w4, logits.shape[-1], coff, _ptr(raw),
+                                                               _ptr(prob), groups, _stream()),
+          "mivos_upsample4x_sigmoid_aggregate_planes")
+    return raw, prob
+
+
 def aggregate_wbg(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False, const_bg: bool = False) -> torch.Tensor:
     _req(prob)
     k = prob.shape[0]
@@ -468,6 +499,44 @@ def aggregate_wbg(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False,
     check(_lib.lib().mivos_aggregate_wbg(_ptr(prob), k, hw, int(keep_bg), int(hard) | (2 if const_bg else 0), _ptr(out), _stream()),
           "mivos_aggregate_wbg")
     return out
+
+
+def aggregate_wbg_planes(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False,
+                         const_bg: bool = False) -> torch.Tensor:
+    """aggregate_wbg for 1 <= K <= MAX_OBJECTS (mivos_aggregate_wbg_planes): the same bits for K <= 16."""
+    _req(prob)
+    k = prob.shape[0]
+    hw = prob[0].numel()
+    out = torch.empty((k + 1 if keep_bg else k,) + tuple(prob.shape[1:]), dtype=torch.float32, device=prob.device)
+    check(_lib.lib().mivos_aggregate_wbg_planes(_ptr(prob), k, hw, int(keep_bg), int(hard) | (2 if const_bg else 0),
+                                                _ptr(out), _stream()), "mivos_aggregate_wbg_planes")
+    return out
+
+
+MAX_OBJECTS = 255           # include/mivos_b200.h: MIVOS_MAX_OBJECTS (the u8 label map)
+REGISTER_AGGREGATE_MAX = 16  # objects the register kernels of upsample4x_sigmoid_aggregate / aggregate_wbg hold
+
+
+def check_objects(k: int, who: str) -> None:
+    """The object counts a clip may have: 1 <= k <= MAX_OBJECTS."""
+    if not 1 <= k <= MAX_OBJECTS:
+        raise _lib.MivosError(f"{who}: {k} objects; 1 to {MAX_OBJECTS} are served (a u8 label map holds {MAX_OBJECTS} "
+                              "objects and the background)")
+
+
+def aggregate_any(prob: torch.Tensor, keep_bg: bool = False, hard: bool = False, const_bg: bool = False) -> torch.Tensor:
+    """aggregate_wbg for any object count: the register kernel up to 16 objects, the plane kernel above."""
+    check_objects(prob.shape[0], "aggregate_wbg")
+    fn = aggregate_wbg if prob.shape[0] <= REGISTER_AGGREGATE_MAX else aggregate_wbg_planes
+    return fn(prob, keep_bg=keep_bg, hard=hard, const_bg=const_bg)
+
+
+def upsample4x_sigmoid_aggregate_any(logits: torch.Tensor, k: int, *a, **kw):
+    """upsample4x_sigmoid_aggregate for any object count: the register kernel up to 16 objects, the plane kernel
+    above."""
+    check_objects(k, "upsample4x_sigmoid_aggregate")
+    fn = upsample4x_sigmoid_aggregate if k <= REGISTER_AGGREGATE_MAX else upsample4x_sigmoid_aggregate_planes
+    return fn(logits, k, *a, **kw)
 
 
 def argmax_unpad(prob: torch.Tensor, pad, h: int, w: int, masks_padded: torch.Tensor,

@@ -15,7 +15,7 @@ import torch.nn as nn
 
 from . import arch, ops
 from . import _lib
-from .engine import PropagationEngine, QueryState, act_dtype_from_env
+from .engine import PropagationEngine, QueryState, act_dtype_from_env, object_chunks
 
 
 class _Reader(nn.Module):
@@ -109,20 +109,25 @@ class PropagationNetwork(nn.Module):
         """memorize() straight into BANK slot `slot` (slot-major keys/values)."""
         eng = self.engine()
         masks = self._f32(masks)
-        K, _, H, W = masks.shape
-        kv = eng.encode_memory(self._f32(frame), masks)
-        ops.bank_write(kv, K, H // 16, W // 16, 0, 128, bank_k, bank_v, slot)
+        ops.check_objects(masks.shape[0], "memorize")
+        eng.memorize_into(self._f32(frame), masks, bank_k, bank_v, slot)
 
     # ------------------------------------------------------------------ reference-layout API
     def memorize(self, frame: torch.Tensor, masks: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-        """prop_net.py:144-162 -> (k16 [K,128,1,h,w], v16 [K,512,1,h,w])."""
+        """prop_net.py:144-162 -> (k16 [K,128,1,h,w], v16 [K,512,1,h,w]); more than 16 objects run in object chunks
+        (engine.object_chunks)."""
         eng = self.engine()
         masks = self._f32(masks)
         K, _, H, W = masks.shape
-        kv = eng.encode_memory(self._f32(frame), masks)
+        ops.check_objects(K, "memorize")
+        frame = self._f32(frame)
         h, w = H // 16, W // 16
-        k16 = ops.halo_to_nchw(kv, K, h, w, 128, coff=0)
-        v16 = ops.halo_to_nchw(kv, K, h, w, 512, coff=128)
+        k16 = torch.empty((K, 128, h, w), dtype=torch.float32, device=masks.device)
+        v16 = torch.empty((K, 512, h, w), dtype=torch.float32, device=masks.device)
+        for k0, n in object_chunks(K):
+            kv = eng.encode_memory(frame, masks, (k0, n))
+            ops.halo_to_nchw(kv, n, h, w, 128, coff=0, out=k16[k0:k0 + n])
+            ops.halo_to_nchw(kv, n, h, w, 512, coff=128, out=v16[k0:k0 + n])
         return k16.unsqueeze(2), v16.unsqueeze(2)
 
     def get_query_values(self, frame: torch.Tensor):
@@ -141,6 +146,7 @@ class PropagationNetwork(nn.Module):
         eng = self.engine()
         keys, values = self._f32(keys), self._f32(values)
         K, _, T, h, w = keys.shape
+        ops.check_objects(K, "segment_with_query")
         H, W = h * 16, w * 16
         dev = keys.device
         slots = T * h * w

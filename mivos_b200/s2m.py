@@ -20,10 +20,10 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import arch
+from . import arch, ops
 from . import _lib
 from ._lib import MivosError
-from .engine import S2MEngine
+from .engine import S2MEngine, object_chunks
 from .tensor_util import pad_divide_by
 
 
@@ -104,10 +104,12 @@ def scribble_inputs(image: torch.Tensor, prev_mask: torch.Tensor, pos: np.ndarra
 
 class S2MController:
     """interact/s2m_controller.py:10-37.  With an ``S2MNetwork`` the K per-object forward passes of the
-    reference loop run as ONE batch of K through the engine (sigmoid fused into the last kernel); any
-    other callable network is called once per object, as the reference loop does."""
+    reference loop run as ONE batch of K through the engine (sigmoid fused into the last kernel), in object chunks
+    of at most 16 above 16 objects (engine.object_chunks); any other callable network is called once per object, as
+    the reference loop does."""
 
     def __init__(self, s2m_net, num_objects: int, ignore_class: int, device="cuda:0"):
+        ops.check_objects(num_objects, "S2MController")
         self.s2m_net = s2m_net
         self.num_objects = num_objects
         self.ignore_class = ignore_class
@@ -121,5 +123,11 @@ class S2MController:
         neg = (scr_mask[None] != ids) & (scr_mask[None] != self.ignore_class)
         x = scribble_inputs(image, prev_mask, pos, neg)
         if isinstance(self.s2m_net, S2MNetwork):
-            return self.s2m_net.forward_sigmoid(x)
+            chunks = object_chunks(self.num_objects)
+            if len(chunks) == 1:
+                return self.s2m_net.forward_sigmoid(x)
+            out = torch.empty((x.shape[0], 1) + tuple(x.shape[-2:]), dtype=torch.float32, device=x.device)
+            for k0, n in chunks:
+                self.s2m_net.forward_sigmoid(x[k0:k0 + n], out=out[k0:k0 + n])
+            return out
         return torch.cat([torch.sigmoid(self.s2m_net(x[i:i + 1])) for i in range(self.num_objects)], 0)
