@@ -213,6 +213,13 @@ MIVOS_API int mivos_halo_to_pixels(const float* halo, int n, int h, int w, int c
 MIVOS_API int mivos_bank_write(const float* halo, int k_objects, int h, int w, int cstride, int coff_k,
                      int coff_v, float* bank_k, float* bank_v, int64_t slots_cap, int t,
                      const int32_t* dyn_t, mivos_stream_t stream);
+/* Per-set form of mivos_bank_write: the K objects are `sets` consecutive sets of K / sets objects (the clips of a
+ * lock-step step), and set s writes bank frame dyn_t[s] (DEVICE array of `sets` int32, read at run time; required).
+ * t_max is the largest frame that may occur (capacity check); a set whose frame lies outside [0, t_max] writes
+ * nothing.  `sets` must divide k_objects.                                                                          */
+MIVOS_API int mivos_bank_write_sets(const float* halo, int k_objects, int sets, int h, int w, int cstride, int coff_k,
+                          int coff_v, float* bank_k, float* bank_v, int64_t slots_cap, int t_max,
+                          const int32_t* dyn_t, mivos_stream_t stream);
 /* Reference-layout bank [K,C,T,h,w] -> BANK (used when a caller hands us torch tensors).        */
 MIVOS_API int mivos_bank_from_nchw(const float* keys, const float* values, int k_objects, int t, int hw,
                          float* bank_k, float* bank_v, int64_t slots_cap, mivos_stream_t stream);
@@ -264,6 +271,30 @@ MIVOS_API int mivos_memory_read_dense(const float* bank_k, const float* bank_v, 
 MIVOS_API int64_t mivos_memory_read_wide_workspace(int k_objects, int64_t slots_cap, int hw, int top_k);
 MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float* bank_v, int64_t slots_cap,
                       int k_objects, int64_t slots, const float* qk, int hw, int q_div, int top_k,
+                      void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
+                      const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
+/* Per-set forms of the three reads: lock-step clips whose banks hold different numbers of live slots.  The
+ * objects are `sets` consecutive sets of k_objects / sets (`sets` must divide k_objects); object o reads query
+ * set o / (k_objects / sets) of qk [sets][hw][128] and the live slots 0 .. dyn_slots[s] - 1 of its own bank, where
+ * dyn_slots is a DEVICE array of `sets` int32 counts read at run time (required).  `slots` (top_k <= slots <=
+ * slots_cap; 1 <= slots for the dense read) sizes the launch and the workspace and bounds no count: each count is
+ * clamped to slots_cap.  Slots at or past a set's count take no part in that set's read (they may hold stale data
+ * or NaN).  Everything else — operands, output window, workspace sizes, topk_idx / topk_val, algo — is that of the
+ * scalar form; with every count equal to n a per-set read gives the bits of the scalar read with dyn_slots = n and
+ * q_div = k_objects / sets.                                                                                        */
+MIVOS_API int mivos_memory_read_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int sets, int top_k,
+                      void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
+                      int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
+MIVOS_API int mivos_memory_read_dense_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int sets,
+                      void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      void* workspace, int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
+                      mivos_stream_t stream);
+MIVOS_API int mivos_memory_read_wide_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int sets, int top_k,
                       void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
                       int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
                       const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);

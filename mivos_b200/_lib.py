@@ -83,9 +83,13 @@ SIGNATURES = {
     "mivos_nchw_to_halo": (_i, [_p, _i, _i, _i, _i, _p, _i, _i, _i, _i, _p]),
     "mivos_halo_to_pixels": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p]),
     "mivos_bank_write": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p, _l, _i, _p, _p]),
+    "mivos_bank_write_sets": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _l, _i, _p, _p]),
     "mivos_bank_from_nchw": (_i, [_p, _p, _i, _i, _i, _p, _p, _l, _p]),
     "mivos_memory_read_workspace": (_l, [_i, _l, _i, _i]),
     "mivos_memory_read": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _i, _p, _i, _p]),
+    "mivos_memory_read_sets": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _i, _p, _i, _p]),
+    "mivos_memory_read_dense_sets": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _i, _i, _i, _p, _l, _p, _i, _p]),
+    "mivos_memory_read_wide_sets": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _p, _i, _p]),
     "mivos_memory_read_stats": (_i, [_p, _i, _l, _i, _i, C.POINTER(_l)]),
     "mivos_memory_read_dense_workspace": (_l, [_i, _l, _i]),
     "mivos_memory_read_dense": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _i, _i, _i, _p, _l, _p, _i, _p]),

@@ -30,12 +30,15 @@ __device__ __forceinline__ void bilin(int dst, float scale, int in_size, int& i0
 }
 
 // ------------------------------------------------------------------------------------------
+// SETS: set s (per_set consecutive objects) writes bank frame dyn_t[s]; a frame outside [0, t] writes nothing
+template <bool SETS>
 __global__ void bank_write_kernel(const float4* __restrict__ halo, int kobj, int h, int w,
                                   int cstride4, int coffk4, int coffv4, float4* __restrict__ bank_k,
                                   float4* __restrict__ bank_v, int64_t slots_cap, int t,
-                                  const int* __restrict__ dyn_t) {
+                                  const int* __restrict__ dyn_t, int per_set) {
   mivos::pdl_prologue();
-  if (dyn_t) t = *dyn_t;  // bank slot from device memory (CUDA-graph replay)
+  const int t_max = t;
+  if (!SETS && dyn_t) t = *dyn_t;  // bank slot from device memory (CUDA-graph replay)
   const int hw = h * w;
   const int per_pix = 32 + 128;  // float4s of key + value
   const int64_t total = static_cast<int64_t>(kobj) * hw * per_pix;
@@ -45,6 +48,10 @@ __global__ void bank_write_kernel(const float4* __restrict__ halo, int kobj, int
     const int64_t t1 = i / per_pix;
     const int p = static_cast<int>(t1 % hw);
     const int obj = static_cast<int>(t1 / hw);
+    if (SETS) {
+      t = dyn_t[obj / per_set];
+      if (t < 0 || t > t_max) continue;
+    }
     const int y = p / w, x = p - y * w;
     const int64_t r = (static_cast<int64_t>(obj) * (h + 2) + y + 1) * (w + 2) + x + 1;
     const int64_t slot = static_cast<int64_t>(t) * hw + p;
@@ -472,9 +479,28 @@ extern "C" MIVOS_API int mivos_bank_write(const float* halo, int k_objects, int 
                     static_cast<int64_t>(t + 1) * h * w <= slots_cap,
                 "bank_write: slot %d does not fit capacity %lld", t, (long long)slots_cap);
   const int64_t total = static_cast<int64_t>(k_objects) * h * w * 160;
-  launch_pdl(bank_write_kernel, capped_grid(total), kThreads, 0, ST(s), 
+  launch_pdl(bank_write_kernel<false>, capped_grid(total), kThreads, 0, ST(s), 
       reinterpret_cast<const float4*>(halo), k_objects, h, w, cstride / 4, coff_k / 4, coff_v / 4,
-      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t, dyn_t);
+      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t, dyn_t, 0);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_bank_write_sets(const float* halo, int k_objects, int sets, int h, int w, int cstride,
+                                               int coff_k, int coff_v, float* bank_k, float* bank_v,
+                                               int64_t slots_cap, int t_max, const int32_t* dyn_t, mivos_stream_t s) {
+  MIVOS_REQUIRE(dyn_t, "bank_write_sets: null frame array (one device-side bank frame per set)");
+  MIVOS_REQUIRE(sets >= 1 && k_objects >= 1 && k_objects % sets == 0, "bank_write_sets: %d sets do not divide %d objects",
+                sets, k_objects);
+  MIVOS_REQUIRE(halo && bank_k && bank_v && AL16(halo) && AL16(bank_k) && AL16(bank_v),
+                "bank_write_sets: null/unaligned pointer");
+  MIVOS_REQUIRE(cstride % 4 == 0 && coff_k % 4 == 0 && coff_v % 4 == 0 && t_max >= 0 &&
+                    static_cast<int64_t>(t_max + 1) * h * w <= slots_cap,
+                "bank_write_sets: slot %d does not fit capacity %lld", t_max, (long long)slots_cap);
+  const int64_t total = static_cast<int64_t>(k_objects) * h * w * 160;
+  launch_pdl(bank_write_kernel<true>, capped_grid(total), kThreads, 0, ST(s),
+      reinterpret_cast<const float4*>(halo), k_objects, h, w, cstride / 4, coff_k / 4, coff_v / 4,
+      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t_max, dyn_t, k_objects / sets);
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }

@@ -84,7 +84,7 @@ memread_exact_kernel(const float* __restrict__ bank_k, int64_t slots_cap, int64_
                      const float* __restrict__ qk_all, int hw, int q_div, int top_k, int tiles_per_split,
                      int splits, int2* __restrict__ cand,
                      int* __restrict__ cand_cnt, const int* __restrict__ flags,
-                     const int* __restrict__ dyn_slots) {
+                     const int* __restrict__ dyn_slots, int dyn_set_stride) {
   mivos::pdl_prologue();
   extern __shared__ __align__(16) uint8_t smem_raw[];
   A1Smem& sm = *reinterpret_cast<A1Smem*>(smem_raw);
@@ -110,7 +110,7 @@ memread_exact_kernel(const float* __restrict__ bank_k, int64_t slots_cap, int64_
   }
   __syncthreads();
 
-  slots = live_slots(dyn_slots, slots, slots_cap);
+  slots = live_slots(dyn_slots, slots, slots_cap, q_div > 0 ? obj / q_div : 0, dyn_set_stride);
   if (dyn_slots) {  // device-side slot count (CUDA-graph replay): fixed grid, ranges derived here
     const int tiles = static_cast<int>((slots + A1_S - 1) / A1_S);
     tiles_per_split = (tiles + splits - 1) / splits;
@@ -491,7 +491,7 @@ int launch_exact_candidates(const MemreadArgs& a, int top_k, const MemreadPlan& 
   dim3 grid(pl.qtiles, pl.splits, a.k_objects);
   launch_pdl(memread_exact_kernel, grid, A1_THREADS, sizeof(A1Smem), stream, a.bank_k, a.slots_cap, a.slots, a.qk, a.hw,
              a.q_div, top_k, pl.tiles_per_split, pl.splits, reinterpret_cast<int2*>(plan_lists(w, pl)),
-             reinterpret_cast<int*>(w + pl.off_cnt), flags, a.dyn_slots);
+             reinterpret_cast<int*>(w + pl.off_cnt), flags, a.dyn_slots, a.dyn_set_stride);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
@@ -532,6 +532,15 @@ int memread_check_args(const MemreadArgs& a, const char* who) {
   return MIVOS_OK;
 }
 
+int memread_sets_args(MemreadArgs& a, int sets, const char* who) {
+  MIVOS_REQUIRE(a.dyn_slots, "%s: null count array (one device-side live slot count per set)", who);
+  MIVOS_REQUIRE(sets >= 1 && a.k_objects >= 1 && a.k_objects % sets == 0,
+                "%s: %d sets do not divide %d objects", who, sets, a.k_objects);
+  a.q_div = a.k_objects / sets;
+  a.dyn_set_stride = 1;
+  return MIVOS_OK;
+}
+
 MemreadWorkspace memread_workspace(int k_objects, int64_t slots, int hw, int top_k) {
   MemreadWorkspace w;
   w.tc = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_TCGEN05);
@@ -556,27 +565,20 @@ extern "C" MIVOS_API int64_t mivos_memory_read_workspace(int k_objects, int64_t 
   return memread_workspace(k_objects, slots, hw, top_k).bytes;
 }
 
-extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* bank_v, int64_t slots_cap,
-                                           int k_objects, int64_t slots, const float* qk, int hw, int q_div,
-                                           int top_k, void* out, int out_cstride, int out_coff,
-                                           int out_halo_h, int out_halo_w, int32_t* topk_idx,
-                                           float* topk_val, void* workspace, int64_t workspace_bytes,
-                                           int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
-                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16};
-  const int rc = memread_check_args(a, "memory_read");
-  if (rc != MIVOS_OK) return rc;
+namespace {
+
+int memory_read_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* topk_val, void* workspace,
+                    int64_t workspace_bytes, int algo, cudaStream_t stream) {
   MIVOS_REQUIRE(top_k >= 1 && top_k <= MAXK, "memory_read: top_k %d outside [1,%d]", top_k, MAXK);
-  MIVOS_REQUIRE(slots >= top_k && slots <= slots_cap && slots < (1ll << 31) - 65536,
-                "memory_read: bad slot count %lld (cap %lld, k %d)", (long long)slots, (long long)slots_cap, top_k);
+  MIVOS_REQUIRE(a.slots >= top_k && a.slots <= a.slots_cap && a.slots < (1ll << 31) - 65536,
+                "memory_read: bad slot count %lld (cap %lld, k %d)", (long long)a.slots, (long long)a.slots_cap, top_k);
   MIVOS_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
                 "memory_read: workspace null or not 256-byte aligned");
-  const int64_t need = mivos_memory_read_workspace(k_objects, slots, hw, top_k);
+  const int64_t need = mivos_memory_read_workspace(a.k_objects, a.slots, a.hw, top_k);
   MIVOS_REQUIRE(workspace_bytes >= need, "memory_read: workspace %lld < %lld bytes", (long long)workspace_bytes, (long long)need);
 
   if (algo == MIVOS_MEMREAD_EXACT_SIMT) {
-    const MemreadPlan pl = memread_plan(k_objects, slots, hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
+    const MemreadPlan pl = memread_plan(a.k_objects, a.slots, a.hw, top_k, MIVOS_MEMREAD_EXACT_SIMT);
     const int rc_a = launch_exact_candidates(a, top_k, pl, workspace, nullptr, stream);
     if (rc_a != MIVOS_OK) return rc_a;
     return launch_select(a, top_k, pl, workspace, nullptr, 0, nullptr, nullptr, nullptr, topk_idx, topk_val, stream);
@@ -585,6 +587,37 @@ extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* ban
     return memread_tc_run(a, top_k, topk_idx, topk_val, workspace, stream);
   set_last_error("memory_read: unknown algo %d", algo);
   return MIVOS_ERR_INVALID;
+}
+
+}  // namespace
+
+extern "C" MIVOS_API int mivos_memory_read(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                           int k_objects, int64_t slots, const float* qk, int hw, int q_div,
+                                           int top_k, void* out, int out_cstride, int out_coff,
+                                           int out_halo_h, int out_halo_w, int32_t* topk_idx,
+                                           float* topk_val, void* workspace, int64_t workspace_bytes,
+                                           int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
+  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
+                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  const int rc = memread_check_args(a, "memory_read");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes, algo,
+                         reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" MIVOS_API int mivos_memory_read_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                int k_objects, int64_t slots, const float* qk, int hw, int sets,
+                                                int top_k, void* out, int out_cstride, int out_coff,
+                                                int out_halo_h, int out_halo_w, int32_t* topk_idx,
+                                                float* topk_val, void* workspace, int64_t workspace_bytes,
+                                                int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
+  MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, 0,
+                out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  int rc = memread_sets_args(a, sets, "memory_read_sets");
+  if (rc == MIVOS_OK) rc = memread_check_args(a, "memory_read_sets");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes, algo,
+                         reinterpret_cast<cudaStream_t>(stream_));
 }
 
 // Debug/diagnostic (synchronises): candidate statistics of the last tensor-core-path read that used

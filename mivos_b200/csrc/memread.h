@@ -40,10 +40,16 @@ struct MemreadArgs {
   // output window: 512 channels at out_coff of rows out_cstride wide; HALO rows when halo_w > 0, else row = obj * hw + q
   void* out;
   int out_cstride, out_coff, halo_h, halo_w, out_f16;
+  // per-set counts (the *_sets entry points): query set s reads dyn_slots[s * dyn_set_stride]; 0: one count for all
+  // (this field fills the struct's tail padding, so the kernels' parameter blocks keep their size)
+  int dyn_set_stride;
 };
 
 // The operand checks both entry points share; `who` prefixes the error text.  MIVOS_OK or MIVOS_ERR_INVALID.
 int memread_check_args(const MemreadArgs& a, const char* who);
+// The per-set form's extra checks (counts given, `sets` divides the objects); sets q_div = objects per set and the
+// count stride.  MIVOS_OK or MIVOS_ERR_INVALID.
+int memread_sets_args(MemreadArgs& a, int sets, const char* who);
 
 struct MemreadPlan {
   int algo;
@@ -100,12 +106,18 @@ __device__ __forceinline__ int float_ordered(float f) {
 }
 __device__ __forceinline__ float ordered_float(int o) { return __int_as_float(o >= 0 ? o : o ^ 0x7fffffff); }
 
-// Live bank slots: the device-side count when there is one, never more than the capacity (the count indexes the bank).
-__device__ __forceinline__ int64_t live_slots(const int* dyn_slots, int64_t slots, int64_t slots_cap) {
-  const int64_t n = dyn_slots ? static_cast<int64_t>(*dyn_slots) : slots;
+// Live bank slots of query set `set`: the device-side count when there is one (dyn_slots[set * set_stride]; stride 0:
+// one count for every set), never more than the capacity (the count indexes the bank).
+__device__ __forceinline__ int64_t live_slots(const int* dyn_slots, int64_t slots, int64_t slots_cap, int set = 0,
+                                              int set_stride = 0) {
+  const int64_t n = dyn_slots ? static_cast<int64_t>(dyn_slots[set * set_stride]) : slots;
   return n < slots_cap ? n : slots_cap;
 }
-__device__ __forceinline__ int64_t live_slots(const MemreadArgs& a) { return live_slots(a.dyn_slots, a.slots, a.slots_cap); }
+// query set of object `obj`
+__device__ __forceinline__ int query_set(const MemreadArgs& a, int obj) { return a.q_div > 0 ? obj / a.q_div : 0; }
+__device__ __forceinline__ int64_t live_slots(const MemreadArgs& a, int obj) {
+  return live_slots(a.dyn_slots, a.slots, a.slots_cap, query_set(a, obj), a.dyn_set_stride);
+}
 
 // The exact score of one key row against a scaled query (q / sqrt(128)): fmaf in ascending channel order.  Every
 // read that selects slots ranks them by this value.  The chain starts at +0, so it never yields -0.

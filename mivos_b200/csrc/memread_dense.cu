@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
   const int q0 = blockIdx.x * DQ;
   const int chunk = blockIdx.y;
   const int obj = blockIdx.z;
-  const int64_t n_live = live_slots(p.a);
+  const int64_t n_live = live_slots(p.a, obj);
   const int64_t live_tiles = (n_live + DS - 1) / DS;
   const int64_t t_begin = static_cast<int64_t>(chunk) * p.chunk_tiles;
   if (t_begin >= live_tiles) return;  // chunk past the live bank: the combine does not read it
@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(32 * C_WARPS) memread_dense_combine_kernel(
   const int hw = a.hw;
   if (lq >= static_cast<int64_t>(a.k_objects) * hw) return;
   const int obj = static_cast<int>(lq / hw), q = static_cast<int>(lq - static_cast<int64_t>(obj) * hw);
-  const int64_t live_tiles = (live_slots(a) + DS - 1) / DS;
+  const int64_t live_tiles = (live_slots(a, obj) + DS - 1) / DS;
   const int live = static_cast<int>((live_tiles + chunk_tiles - 1) / chunk_tiles);
   const int64_t base = static_cast<int64_t>(obj) * chunks * hw + q;  // chunk c of this query: base + c * hw
   float M = -INFINITY;
@@ -338,16 +338,11 @@ extern "C" MIVOS_API int64_t mivos_memory_read_dense_workspace(int k_objects, in
   return dense_plan(k_objects, slots_cap, hw).bytes;
 }
 
-extern "C" MIVOS_API int mivos_memory_read_dense(const float* bank_k, const float* bank_v, int64_t slots_cap,
-                                                 int k_objects, int64_t slots, const float* qk, int hw, int q_div,
-                                                 void* out, int out_cstride, int out_coff, int out_halo_h,
-                                                 int out_halo_w, void* workspace, int64_t workspace_bytes,
-                                                 const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
-                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16};
-  const int rc = memread_check_args(a, "memory_read_dense");
-  if (rc != MIVOS_OK) return rc;
+namespace {
+
+int memory_read_dense_run(const MemreadArgs& a, void* workspace, int64_t workspace_bytes, cudaStream_t stream) {
+  const int64_t slots_cap = a.slots_cap, slots = a.slots;
+  const int k_objects = a.k_objects, hw = a.hw;
   MIVOS_REQUIRE(slots_cap >= 1 && slots_cap < (1ll << 31) - 65536 && slots >= 1 && slots <= slots_cap,
                 "memory_read_dense: bad slot count %lld (cap %lld)", (long long)slots, (long long)slots_cap);
   MIVOS_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
@@ -379,4 +374,31 @@ extern "C" MIVOS_API int mivos_memory_read_dense(const float* bank_k, const floa
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
+}
+
+}  // namespace
+
+extern "C" MIVOS_API int mivos_memory_read_dense(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                 int k_objects, int64_t slots, const float* qk, int hw, int q_div,
+                                                 void* out, int out_cstride, int out_coff, int out_halo_h,
+                                                 int out_halo_w, void* workspace, int64_t workspace_bytes,
+                                                 const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
+  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
+                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  const int rc = memread_check_args(a, "memory_read_dense");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_dense_run(a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" MIVOS_API int mivos_memory_read_dense_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                      int k_objects, int64_t slots, const float* qk, int hw, int sets,
+                                                      void* out, int out_cstride, int out_coff, int out_halo_h,
+                                                      int out_halo_w, void* workspace, int64_t workspace_bytes,
+                                                      const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
+  MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, 0,
+                out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  int rc = memread_sets_args(a, sets, "memory_read_dense_sets");
+  if (rc == MIVOS_OK) rc = memread_check_args(a, "memory_read_dense_sets");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_dense_run(a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }

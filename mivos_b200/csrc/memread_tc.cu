@@ -75,9 +75,8 @@ __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_
                                     float* __restrict__ qnorm, const float* __restrict__ bank_k,
                                     int64_t slots_cap, int64_t slots, int k_objects,
                                     unsigned int* __restrict__ kmax2_bits, int qblocks,
-                                    const int* __restrict__ dyn_slots, int* __restrict__ tau_g) {
+                                    const int* __restrict__ dyn_slots, int dyn_set_stride, int* __restrict__ tau_g) {
   mivos::pdl_prologue();
-  slots = live_slots(dyn_slots, slots, slots_cap);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (static_cast<int>(blockIdx.x) < qblocks) {
     // one warp per query row r = set * hw + q
@@ -104,8 +103,10 @@ __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_
   const int nb = gridDim.x - qblocks;
   const int b = blockIdx.x - qblocks;
   for (int obj = 0; obj < k_objects; ++obj) {
+    // the bound covers the live keys of this object's set only
+    const int64_t live = live_slots(dyn_slots, slots, slots_cap, q_div > 0 ? obj / q_div : 0, dyn_set_stride);
     float best = 0.f;
-    for (int64_t s = static_cast<int64_t>(b) * 8 + warp; s < slots; s += static_cast<int64_t>(nb) * 8) {
+    for (int64_t s = static_cast<int64_t>(b) * 8 + warp; s < live; s += static_cast<int64_t>(nb) * 8) {
       const float4 v = reinterpret_cast<const float4*>(bank_k + (static_cast<int64_t>(obj) * slots_cap + s) * 128)[lane];
       float n2 = v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
 #pragma unroll
@@ -214,7 +215,9 @@ constexpr int STG_BYTES = 64 * STG_STRIDE * 4;
 // each); 9 warps put 3 on one partition, so 16384 / (3 x 32) caps a thread at 168 — a larger cap compiles but the
 // launch is refused.  The 128-float accumulator fragment, the NB bucket maxima and a 32-score chunk do not all fit
 // there: ptxas spills 0.3-1.3 KB per thread (NB = 32 / 64), served from L1, inside the candidate loop.
-template <int NB>
+// SETS: per-set counts (query set s reads its count from dyn_slots[s]).  A template flag, not a TcParams field, so
+// the scalar instantiations keep their parameter block and register allocation.
+template <int NB, bool SETS>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                   const TcParams p) {
@@ -235,8 +238,9 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const int q0 = blockIdx.x * TQ;
   const int split = blockIdx.y;
   const int obj = blockIdx.z;
-  const int qrow0 = (p.q_div > 0 ? obj / p.q_div : 0) * p.hw;  // first row of this object's query set
-  const int64_t slots = live_slots(p.dyn_slots, p.slots, p.slots_cap);
+  const int qset = p.q_div > 0 ? obj / p.q_div : 0;
+  const int qrow0 = qset * p.hw;  // first row of this object's query set
+  const int64_t slots = live_slots(p.dyn_slots, p.slots, p.slots_cap, SETS ? qset : 0, SETS ? 1 : 0);
   const int total_tiles = static_cast<int>((slots + TS - 1) / TS);
   // with a device-side slot count the grid (splits) is fixed by the host for the bank capacity and
   // the tile ranges are derived here; splits beyond the live bank publish empty lists and leave
@@ -479,7 +483,7 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
   const int qblocks = ceil_div(q_rows, 8);
   const int kblocks = 296;
   launch_pdl(memread_prep_kernel, qblocks + kblocks, 256, 0, stream, a.qk, a.hw, q_rows, a.q_div, qs, qnorm, a.bank_k,
-             a.slots_cap, a.slots, a.k_objects, kmax2, qblocks, a.dyn_slots, tau_g);
+             a.slots_cap, a.slots, a.k_objects, kmax2, qblocks, a.dyn_slots, a.dyn_set_stride, tau_g);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 
@@ -509,13 +513,18 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
 
   static bool configured = false;
   if (!configured) {
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
     configured = true;
   }
   dim3 grid(tc.qtiles, tc.splits, a.k_objects);
-  if (top_k <= 32) launch_pdl(memread_tc_kernel<32>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-  else launch_pdl(memread_tc_kernel<64>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  const bool sets = a.dyn_set_stride != 0;
+  if (top_k <= 32 && !sets) launch_pdl(memread_tc_kernel<32, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  else if (!sets) launch_pdl(memread_tc_kernel<64, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  else if (top_k <= 32) launch_pdl(memread_tc_kernel<32, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  else launch_pdl(memread_tc_kernel<64, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 

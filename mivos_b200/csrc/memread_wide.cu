@@ -98,7 +98,7 @@ memread_wide_sweep_kernel(const MemreadArgs a, const int splits, const WideState
     sm.qT[c][q] = q < nq ? qk[static_cast<int64_t>(q) * 128 + c] / kSqrtCK : 0.f;  // prop_net.py:86
   }
 
-  const int64_t live = live_slots(a);
+  const int64_t live = live_slots(a, obj);
   const int64_t tiles = (live + WS - 1) / WS;
   const float* keys = a.bank_k + static_cast<int64_t>(obj) * a.slots_cap * 128;
   const int tq = tid & 15, ts = tid >> 4;
@@ -355,7 +355,7 @@ memread_wide_select_kernel(const MemreadArgs a, const int top_k, const WideState
   const int hw = a.hw;
   const int obj = static_cast<int>(lq / hw), q = static_cast<int>(lq - static_cast<int64_t>(obj) * hw);
   const int qset = a.q_div > 0 ? obj / a.q_div : 0;
-  const int64_t live = live_slots(a);
+  const int64_t live = live_slots(a, obj);
 
   int n;
   if (state[lq].mode != 2) {
@@ -473,23 +473,16 @@ extern "C" MIVOS_API int64_t mivos_memory_read_wide_workspace(int k_objects, int
   return wide_plan(k_objects, hw).bytes;
 }
 
-extern "C" MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float* bank_v, int64_t slots_cap,
-                                                int k_objects, int64_t slots, const float* qk, int hw, int q_div,
-                                                int top_k, void* out, int out_cstride, int out_coff, int out_halo_h,
-                                                int out_halo_w, int32_t* topk_idx, float* topk_val, void* workspace,
-                                                int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
-                                                mivos_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
-                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16};
-  const int rc = memread_check_args(a, "memory_read_wide");
-  if (rc != MIVOS_OK) return rc;
+namespace {
+
+int memory_read_wide_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* topk_val, void* workspace,
+                         int64_t workspace_bytes, cudaStream_t stream) {
   MIVOS_REQUIRE(top_k >= 1 && top_k <= kWideMaxK, "memory_read_wide: top_k %d outside [1,%d]", top_k, kWideMaxK);
-  MIVOS_REQUIRE(slots >= top_k && slots <= slots_cap && slots_cap < (1ll << 31) - 65536,
-                "memory_read_wide: bad slot count %lld (cap %lld, k %d)", (long long)slots, (long long)slots_cap, top_k);
+  MIVOS_REQUIRE(a.slots >= top_k && a.slots <= a.slots_cap && a.slots_cap < (1ll << 31) - 65536,
+                "memory_read_wide: bad slot count %lld (cap %lld, k %d)", (long long)a.slots, (long long)a.slots_cap, top_k);
   MIVOS_REQUIRE(workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
                 "memory_read_wide: workspace null or not 256-byte aligned");
-  const WidePlan pl = wide_plan(k_objects, hw);
+  const WidePlan pl = wide_plan(a.k_objects, a.hw);
   MIVOS_REQUIRE(workspace_bytes >= pl.bytes, "memory_read_wide: workspace %lld < %lld bytes", (long long)workspace_bytes,
                 (long long)pl.bytes);
 
@@ -509,11 +502,11 @@ extern "C" MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float
   int* cnt = reinterpret_cast<int*>(w + pl.off_cnt);
   WideState* state = reinterpret_cast<WideState*>(w + pl.off_state);
   int2* cand = reinterpret_cast<int2*>(w + pl.off_cand);
-  const int64_t nq = static_cast<int64_t>(k_objects) * hw;
+  const int64_t nq = static_cast<int64_t>(a.k_objects) * a.hw;
 
   // histogram and emission counts start at zero (adjacent: one memset); the level-1 threshold clears each row it reads
   MIVOS_CUDA_OK(cudaMemsetAsync(w, 0, static_cast<size_t>(pl.off_state), stream));
-  const dim3 grid(pl.qtiles, pl.splits, k_objects);
+  const dim3 grid(pl.qtiles, pl.splits, a.k_objects);
   const int tblocks = static_cast<int>(ceil_div64(nq, 8));
   launch_pdl(memread_wide_sweep_kernel<0>, grid, W_THREADS, hist_smem, stream, a, pl.splits,
              static_cast<const WideState*>(state), hist, cand, cnt);
@@ -529,4 +522,35 @@ extern "C" MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float
   g_launches.fetch_add(6, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
+}
+
+}  // namespace
+
+extern "C" MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                int k_objects, int64_t slots, const float* qk, int hw, int q_div,
+                                                int top_k, void* out, int out_cstride, int out_coff, int out_halo_h,
+                                                int out_halo_w, int32_t* topk_idx, float* topk_val, void* workspace,
+                                                int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
+                                                mivos_stream_t stream_) {
+  const MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, q_div,
+                      out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  const int rc = memread_check_args(a, "memory_read_wide");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_wide_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes,
+                              reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" MIVOS_API int mivos_memory_read_wide_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                     int k_objects, int64_t slots, const float* qk, int hw, int sets,
+                                                     int top_k, void* out, int out_cstride, int out_coff, int out_halo_h,
+                                                     int out_halo_w, int32_t* topk_idx, float* topk_val, void* workspace,
+                                                     int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
+                                                     mivos_stream_t stream_) {
+  MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, 0,
+                out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  int rc = memread_sets_args(a, sets, "memory_read_wide_sets");
+  if (rc == MIVOS_OK) rc = memread_check_args(a, "memory_read_wide_sets");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_wide_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes,
+                              reinterpret_cast<cudaStream_t>(stream_));
 }

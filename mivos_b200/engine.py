@@ -50,9 +50,27 @@ class Workspace:
         self.device = device
         self.dtype = dtype  # element type of activation maps (fp32 for the TF32 path, or fp16)
         self._bufs: Dict[tuple, torch.Tensor] = {}
+        self._prefix = None  # (n, full) inside prefix_of()
+
+    @contextlib.contextmanager
+    def prefix_of(self, n: int, full: int):
+        """Inside the block, a buffer of n maps (a HALO map of n images, a matrix of n images' rows) is the leading
+        part of the buffer of `full` maps: a batch of the first n of `full` lock-step clips allocates nothing the
+        full batch does not.  HALO maps and gathered matrices are image-major, so the prefix is contiguous."""
+        prev, self._prefix = self._prefix, (n, full)
+        try:
+            yield
+        finally:
+            self._prefix = prev
+
+    def full(self, n: int) -> int:
+        """The map count a buffer of n maps is allocated for (see prefix_of)."""
+        return self._prefix[1] if self._prefix is not None and n == self._prefix[0] else n
 
     def halo(self, tag: str, n: int, h: int, w: int, c: int, dtype=None) -> torch.Tensor:
         dtype = dtype or self.dtype
+        if self._prefix is not None and n == self._prefix[0] and n != self._prefix[1]:
+            return self.halo(tag, self._prefix[1], h, w, c, dtype)[:n]
         key = ("halo", tag, n, h, w, c, dtype)
         buf = self._bufs.get(key)
         if buf is None:
@@ -62,6 +80,13 @@ class Workspace:
 
     def mat(self, tag: str, rows: int, cols: int, dtype=None) -> torch.Tensor:
         dtype = dtype or self.dtype
+        if self._prefix is not None and self._prefix[0] != self._prefix[1] and rows % self._prefix[0] == 0:
+            full = rows // self._prefix[0] * self._prefix[1]
+            prev, self._prefix = self._prefix, None  # the full-size lookup itself
+            try:
+                return self.mat(tag, full, cols, dtype)[:rows]
+            finally:
+                self._prefix = prev
         key = ("mat", tag, rows, cols, dtype)
         buf = self._bufs.get(key)
         if buf is None:
@@ -362,11 +387,17 @@ class PropagationEngine(_ResNetTrunk):
         _cg(self.ws, f16, self.pc["kv_m_f16"], N, h16, w16, kv)
         return kv
 
-    def memorize_into(self, frames: torch.Tensor, masks: torch.Tensor, bank_k, bank_v, t: int, dyn_t=None) -> None:
+    def memorize_into(self, frames: torch.Tensor, masks: torch.Tensor, bank_k, bank_v, t: int, dyn_t=None,
+                      dyn_sets: bool = False) -> None:
         """encode_memory + bank_write into bank frame `t` (or the device scalar dyn_t, t its largest value) for every
-        object: C clips of K <= CHUNK_OBJECTS objects in one batch, one clip of more objects in object_chunks."""
+        object: C clips of K <= CHUNK_OBJECTS objects in one batch, one clip of more objects in object_chunks.
+        dyn_sets (C clips, masks [C,K,1,H,W]): dyn_t holds one frame per clip, clip c writes frame dyn_t[c]."""
         H, W = masks.shape[-2:]
         N = masks.shape[:-3].numel()
+        if dyn_sets:
+            kv = self.encode_memory(frames, masks)
+            ops.bank_write_sets(kv, N, masks.shape[0], H // 16, W // 16, 0, 128, bank_k, bank_v, t, dyn_t)
+            return
         for k0, n in ([(0, N)] if masks.dim() == 5 else object_chunks(N)):
             kv = self.encode_memory(frames, masks, (k0, n))
             ops.bank_write(kv, n, H // 16, W // 16, 0, 128, bank_k[k0:k0 + n], bank_v[k0:k0 + n], t, dyn_t=dyn_t)
@@ -391,11 +422,28 @@ class PropagationEngine(_ResNetTrunk):
         """Fewest live bank slots a read accepts: top_k for the top-k read (as torch.topk), 1 for the dense read."""
         return 1 if self.top_k is None else self.top_k
 
-    def _memory_read(self, bank_k, bank_v, slots: int, qk, n: int, cat, h16: int, w16: int, dyn_slots, q_div: int):
+    def _memory_read(self, bank_k, bank_v, slots: int, qk, n: int, cat, h16: int, w16: int, dyn_slots, q_div: int,
+                     dyn_sets: bool = False):
         """The memory read of n objects into channels [0, 512) of `cat`: the top-k read (prop_net.py:47-73) for
         top_k <= 64, the wide top-k read above that, or the dense read of the reference's top_k=None
-        (prop_net.py:99-102).  The only place that tells them apart."""
+        (prop_net.py:99-102).  The only place that tells them apart.  dyn_sets: qk [sets,hw,128] and one live slot
+        count per set in dyn_slots (the per-set forms)."""
         hw = h16 * w16
+        if dyn_sets:
+            nf = self.ws.full(n)  # a prefix batch reads through the full batch's workspace
+            if self.top_k is None:
+                wsp = self.ws.raw("memread_dense", ops.memory_read_dense_workspace_bytes(nf, bank_k.shape[1], hw))
+                ops.memory_read_dense_sets(bank_k, bank_v, slots, qk, cat, dyn_slots, halo_hw=(h16, w16), workspace=wsp)
+            elif self.top_k > ops.TOPK_READ_MAX_K:
+                wsp = self.ws.raw("memread_wide",
+                                  ops.memory_read_wide_workspace_bytes(nf, bank_k.shape[1], hw, self.top_k))
+                ops.memory_read_wide_sets(bank_k, bank_v, slots, qk, self.top_k, cat, dyn_slots, halo_hw=(h16, w16),
+                                          workspace=wsp)
+            else:
+                wsp = self.ws.raw("memread", ops.memory_read_workspace_bytes(nf, slots, hw, self.top_k))
+                ops.memory_read_sets(bank_k, bank_v, slots, qk, self.top_k, cat, dyn_slots, halo_hw=(h16, w16),
+                                     workspace=wsp, algo=self.memread_algo)
+            return
         if self.top_k is None:
             wsp = self.ws.raw("memread_dense", ops.memory_read_dense_workspace_bytes(n, bank_k.shape[1], hw))
             ops.memory_read_dense(bank_k, bank_v, slots, qk, cat, out_coff=0, halo_hw=(h16, w16), workspace=wsp,
@@ -413,7 +461,7 @@ class PropagationEngine(_ResNetTrunk):
                             algo=self.memread_algo, dyn_slots=dyn_slots, q_div=q_div)
 
     def segment(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int = 1, *, prob_out=None, want_raw=False,
-                want_prob=True, dyn_slots=None):
+                want_prob=True, dyn_slots=None, dyn_sets: bool = False):
         """segment_with_query (prop_net.py:170-181) + aggregate_wbg(keep_bg=True) (inference_core.py:175) for C
         clips.  The C*K object maps (clip-major: map c*K + k is object k of clip c) go through every convolution as
         ONE batch — the 1/16- and 1/8-resolution layers of a single clip have 14-54 row tiles for 132 SMs — while the
@@ -422,10 +470,13 @@ class PropagationEngine(_ResNetTrunk):
         (object_chunks), each chunk writing its slice of one K-object logits map; one aggregation over all K follows.
         bank_k/bank_v [C*K, cap, 128/512]; `q` the QueryState of one clip's frame, or for C > 1 the batched state of
         the C current frames (new_query_states(H, W, C)).  Returns (raw sigmoid [C*K,1,H,W] | None, prob
-        [(K+1),1,H,W] | None), prob [C,K+1,1,H,W] for C > 1."""
+        [(K+1),1,H,W] | None), prob [C,K+1,1,H,W] for C > 1.  dyn_sets: `q` is a batched state of C >= 1 clips and
+        dyn_slots holds one live slot count per clip (the per-set read)."""
         H, W = q.h, q.w
         chunks = object_chunks(K) if C == 1 else [(0, K)]
-        if len(chunks) == 1:
+        if dyn_sets:
+            lg = self._decode(bank_k, bank_v, slots, q, K, C, dyn_slots, None, dyn_sets=True)
+        elif len(chunks) == 1:
             lg = self._decode(bank_k, bank_v, slots, q, K, C, dyn_slots, None)
         else:
             lg = self.ws.halo("logit", K, H // 4, W // 4, 32, torch.float32)
@@ -434,7 +485,7 @@ class PropagationEngine(_ResNetTrunk):
         return ops.upsample4x_sigmoid_aggregate_any(lg, K, H // 4, W // 4, want_raw=want_raw, want_prob=want_prob,
                                                     prob_out=prob_out, groups=C)
 
-    def _decode(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int, dyn_slots, lg):
+    def _decode(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int, dyn_slots, lg, dyn_sets: bool = False):
         """Memory read and decoder of C*K object maps as one batch; returns their decoder.pred logits in `lg` (a
         workspace map when None)."""
         ws, pc = self.ws, self.pc
@@ -443,7 +494,7 @@ class PropagationEngine(_ResNetTrunk):
         N = C * K
         cat = ws.halo("cat", N, h16, w16, 1024)
         # ONE read for the C clips: object c*K + k reads query set c (q_div = K objects per set; one clip: q_div 0)
-        self._memory_read(bank_k, bank_v, slots, q.qk, N, cat, h16, w16, dyn_slots, K if C > 1 else 0)
+        self._memory_read(bank_k, bank_v, slots, q.qk, N, cat, h16, w16, dyn_slots, K if C > 1 else 0, dyn_sets)
         ops.halo_copy(q.kv, cat, N, h16, w16, 512, src_coff=128, dst_coff=512)  # cat([readout, v16]) :178-179
         catr = ws.halo("catr", N, h16, w16, 1024)
         ops.halo_copy(cat, catr, N, h16, w16, 1024, relu=True)

@@ -24,7 +24,7 @@ class FrameStep:
     cached on the network's engine and shared by successive sessions — the reference also shares the networks between
     sessions (eval_interactive_davis.py:83)."""
 
-    def __init__(self, net, C: int, K: int, nh: int, nw: int, cap_frames: int, lane: int = 0):
+    def __init__(self, net, C: int, K: int, nh: int, nw: int, cap_frames: int, lane: int = 0, ragged: bool = False):
         eng = net.engine()
         dev = eng.device
         # the step is cached on the network's engine: a strong reference back would be a cycle that keeps a dropped
@@ -59,20 +59,25 @@ class FrameStep:
         self.s_fixed = i64([self.prob[c, j].data_ptr() for c in range(C) for j in range(K + 1)])
         self.plane_bytes = nh * nw * 4
         self.s_bytes = i64([self.plane_bytes] * (C * (K + 1)))
-        self.dynp = torch.zeros(C * (6 + K), dtype=torch.int64, device=dev)
+        # ragged (clips with their own pass plans, LockstepSession): C more words of the table hold one live slot
+        # count and one memorize frame per clip, as int32 `counts` [2C] = (slots of clips 0..C-1, frames of clips
+        # 0..C-1), written with the pointers; a tick of the first n of the C clips runs over their leading rows
+        self.ragged = ragged
+        self.dynp = torch.zeros(C * (6 + K) + (C if ragged else 0), dtype=torch.int64, device=dev)
+        self.counts = self.dynp[C * (6 + K):].view(torch.int32) if ragged else None
 
     @staticmethod
-    def get(net, C: int, K: int, nh: int, nw: int, need_frames: int, lane: int = 0) -> "FrameStep":
+    def get(net, C: int, K: int, nh: int, nw: int, need_frames: int, lane: int = 0, ragged: bool = False) -> "FrameStep":
         """The cached step for these shapes.  Single clips are kept in the engine's `_frame_steps` (4 entries),
         lock-step groups, whose C*K banks are C times larger, in `_lock_steps` (2 entries); least recently used
         first out."""
         name, bound = ("_frame_steps", 4) if C == 1 else ("_lock_steps", 2)
         cache = net.engine().__dict__.setdefault(name, {})
         cap = (need_frames + 15) // 16 * 16
-        key = (C, K, nh, nw, cap, lane)
+        key = (C, K, nh, nw, cap, lane) + (("ragged",) if ragged else ())
         step = cache.pop(key, None)
         if step is None:
-            step = FrameStep(net, C, K, nh, nw, cap, lane)
+            step = FrameStep(net, C, K, nh, nw, cap, lane, ragged)
             while len(cache) >= bound:  # dict order = use order
                 cache.pop(next(iter(cache)))
         cache[key] = step  # (re)insert as most recently used
@@ -89,6 +94,79 @@ class FrameStep:
                 eng.memorize_into(self.frames, self.masks, self.bank_k, self.bank_v, self.cap_frames - 1,
                                   dyn_t=self.dyn[1:2])
             ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, C * (K + 1), False, self.plane_bytes)
+
+    def _body_ragged(self, n: int, n_mem: int):
+        """A tick of the first n clips, the first n_mem of them memorizing: the same operators as _body over the
+        leading n (n_mem) clips, the reads and the bank write in their per-set forms (counts per clip)."""
+        eng, C, K = self.net.engine(), self.C, self.K
+        with eng.lane(self.lane):
+            ws = eng.ws
+            ops.copy_segments(self.g_fixed, self.dynp, self.g_bytes, 5 * n, True, max(self.g_bytes_host))
+            with ws.prefix_of(n * K, C * K):
+                eng.segment(self.bank_k[:n * K], self.bank_v[:n * K], self.cap_frames * self.hw, self.batch.first(n), K,
+                            n, prob_out=self.prob[0] if n == 1 else self.prob[:n], dyn_slots=self.counts[:n],
+                            dyn_sets=True)
+            if n_mem:
+                with ws.prefix_of(n_mem * K, C * K):
+                    eng.memorize_into(self.frames[:n_mem], self.prob[:n_mem].narrow(-4, 1, K), self.bank_k[:n_mem * K],
+                                      self.bank_v[:n_mem * K], self.cap_frames - 1, dyn_t=self.counts[C:C + n_mem],
+                                      dyn_sets=True)
+            ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, n * (K + 1), False, self.plane_bytes)
+
+    def run_ragged(self, frames: Sequence[Optional[torch.Tensor]], cached, visible: Sequence[int],
+                   m_front: Sequence[int], n_mem: int, prob_dsts, ti: Sequence[int], graph: bool = True) -> torch.Tensor:
+        """One tick of the first n = len(cached) clips of a ragged step, each at its own frame: clip c reads
+        visible[c] bank frames and (c < n_mem) memorizes into frame m_front[c]; frames[c] / cached[c] / ti[c] as in
+        run, prob_dsts[c] clip c's destination volume or None (fused frame: the planes stay in self.prob[c]).  The
+        pointers and the per-clip counters are written with one store; one captured graph per (n, n_mem)."""
+        assert self.ragged
+        n, C, K = len(cached), self.C, self.K
+        assert 1 <= n <= C and 0 <= n_mem <= n
+        srcs, dsts, slots, mem_t = [], [], [], []
+        for c in range(C):
+            if c < n:
+                assert visible[c] <= self.cap_frames and m_front[c] < self.cap_frames
+                if visible[c] * self.hw < self.net.min_live_slots:  # same rule as mivos_memory_read and torch.topk
+                    raise MivosError(f"memory_read: clip {c}: {visible[c] * self.hw} live bank slots < top_k "
+                                     f"{self.net.top_k}")
+                q = cached[c]
+                srcs += [frames[c].data_ptr() if c < n_mem else 0, q.kv.data_ptr(), q.qk.data_ptr(), q.s8.data_ptr(),
+                         q.s4.data_ptr()]
+                d = prob_dsts[c]
+                dsts += [d[j, ti[c]].data_ptr() for j in range(K + 1)] if d is not None else [0] * (K + 1)
+                slots.append(visible[c] * self.hw)
+                mem_t.append(m_front[c] if c < n_mem else 0)
+            else:
+                srcs += [0] * 5
+                dsts += [0] * (K + 1)
+                slots.append(0)
+                mem_t.append(0)
+        i32 = slots + mem_t
+        packed = [(i32[2 * i] & 0xFFFFFFFF) | ((i32[2 * i + 1] & 0xFFFFFFFF) << 32) for i in range(C)]
+        packed = [w - (1 << 64) if w >= 1 << 63 else w for w in packed]
+        ops.store_words(self.dynp, srcs + dsts + packed)
+        if not (graph and self.use_graph):
+            self._body_ragged(n, n_mem)
+            return self.prob
+        lib = _lib.load()
+        key = (n, n_mem)
+        g = self.graphs.get(key)
+        if g is None:
+            n0 = lib.mivos_launch_count()
+            self._body_ragged(n, n_mem)
+            self.kernels[key] = lib.mivos_launch_count() - n0
+            torch.cuda.current_stream().synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._body_ragged(n, n_mem)
+            lib.mivos_add_launch_count(-self.kernels[key])
+            self.graphs[key] = g
+            # the eager run above was this tick: a replay would run it twice, and a prefix first appears mid-pass,
+            # where a clip's read may see the temporary bank frame its memorize has just overwritten
+            return self.prob
+        g.replay()
+        lib.mivos_add_launch_count(self.kernels[key])
+        return self.prob
 
     def run(self, frames: Sequence[Optional[torch.Tensor]], cached, visible: int, m_front: int, memorize: bool,
             prob_dsts=None, ti: int = 0, graph: bool = True) -> torch.Tensor:

@@ -342,6 +342,16 @@ def bank_write(halo: torch.Tensor, k: int, h: int, w: int, coff_k: int, coff_v: 
                                       _ptr(bank_v), bank_k.shape[1], t, _ptr(dyn_t), _stream()), "mivos_bank_write")
 
 
+def bank_write_sets(halo: torch.Tensor, k: int, sets: int, h: int, w: int, coff_k: int, coff_v: int,
+                    bank_k: torch.Tensor, bank_v: torch.Tensor, t_max: int, dyn_t: torch.Tensor) -> None:
+    """bank_write of `sets` sets of k // sets objects (lock-step clips), set s into bank frame dyn_t[s] (int32 device
+    array, read when the launch runs); `t_max` is the largest frame that may occur."""
+    _req(halo), _req(bank_k), _req(bank_v), _req(dyn_t, torch.int32)
+    check(_lib.lib().mivos_bank_write_sets(_ptr(halo), k, sets, h, w, halo.shape[-1], coff_k, coff_v, _ptr(bank_k),
+                                           _ptr(bank_v), bank_k.shape[1], t_max, _ptr(dyn_t), _stream()),
+          "mivos_bank_write_sets")
+
+
 def bank_from_nchw(keys: torch.Tensor, values: torch.Tensor, bank_k: torch.Tensor, bank_v: torch.Tensor) -> None:
     """keys [K,128,T,h,w], values [K,512,T,h,w] (reference layout) -> BANK."""
     _req(keys), _req(values), _req(bank_k), _req(bank_v)
@@ -395,6 +405,27 @@ def memory_read(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torc
     return (out, idx, val) if want_topk else out
 
 
+def memory_read_sets(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, top_k: int,
+                     out: torch.Tensor, counts: torch.Tensor, *, out_coff: int = 0, halo_hw=None,
+                     workspace: Optional[torch.Tensor] = None, algo: int = MEMREAD_AUTO, want_topk: bool = False):
+    """memory_read of lock-step clips with banks of different fill: object o reads query set s = o // (k / sets) of qk
+    [sets,hw,128] over the live slots 0 .. counts[s] - 1 of its bank (counts: int32 device [sets], read when the
+    launch runs).  `slots` (>= top_k, <= capacity) sizes the launch and the workspace."""
+    sets = _set_counts("memory_read_sets", qk, counts)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_sets", bank_k, bank_v, qk, out, -(-bank_k.shape[0] // sets), halo_hw, workspace,
+        lambda k, cap, hw: memory_read_workspace_bytes(k, slots, hw, top_k))
+    idx = val = None
+    if want_topk:
+        idx = torch.empty((k, hw, top_k), dtype=torch.int32, device=qk.device)
+        val = torch.empty((k, hw, top_k), dtype=torch.float32, device=qk.device)
+    check(_lib.lib().mivos_memory_read_sets(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, sets, top_k,
+                                            _ptr(out), out.shape[-1], out_coff, hh, ww, _ptr(idx), _ptr(val),
+                                            _ptr(workspace), workspace.numel(), algo, _ptr(counts), _f16(out), _stream()),
+          "mivos_memory_read_sets")
+    return (out, idx, val) if want_topk else out
+
+
 def memory_read_dense_workspace_bytes(k: int, slots_cap: int, hw: int) -> int:
     """Workspace of memory_read_dense for k objects over a bank of `slots_cap` slots (the capacity, not the live count)."""
     n = _lib.load().mivos_memory_read_dense_workspace(k, slots_cap, hw)
@@ -414,6 +445,21 @@ def memory_read_dense(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk
                                              out.shape[-1], out_coff, hh, ww, _ptr(workspace), workspace.numel(),
                                              _ptr(dyn_slots), _f16(out), _stream()),
           "mivos_memory_read_dense")
+    return out
+
+
+def memory_read_dense_sets(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor,
+                           out: torch.Tensor, counts: torch.Tensor, *, out_coff: int = 0, halo_hw=None,
+                           workspace: Optional[torch.Tensor] = None):
+    """memory_read_dense with one live slot count per query set, as memory_read_sets."""
+    sets = _set_counts("memory_read_dense_sets", qk, counts)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_dense_sets", bank_k, bank_v, qk, out, -(-bank_k.shape[0] // sets), halo_hw, workspace,
+        memory_read_dense_workspace_bytes)
+    check(_lib.lib().mivos_memory_read_dense_sets(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, sets,
+                                                  _ptr(out), out.shape[-1], out_coff, hh, ww, _ptr(workspace),
+                                                  workspace.numel(), _ptr(counts), _f16(out), _stream()),
+          "mivos_memory_read_dense_sets")
     return out
 
 
@@ -449,6 +495,34 @@ def memory_read_wide(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk:
                                             _stream()),
           "mivos_memory_read_wide")
     return (out, idx, val) if want_topk else out
+
+
+def memory_read_wide_sets(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, top_k: int,
+                          out: torch.Tensor, counts: torch.Tensor, *, out_coff: int = 0, halo_hw=None,
+                          workspace: Optional[torch.Tensor] = None, want_topk: bool = False):
+    """memory_read_wide with one live slot count per query set, as memory_read_sets."""
+    sets = _set_counts("memory_read_wide_sets", qk, counts)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_wide_sets", bank_k, bank_v, qk, out, -(-bank_k.shape[0] // sets), halo_hw, workspace,
+        lambda k, cap, hw: memory_read_wide_workspace_bytes(k, cap, hw, top_k))
+    idx = val = None
+    if want_topk:
+        idx = torch.empty((k, hw, top_k), dtype=torch.int32, device=qk.device)
+        val = torch.empty((k, hw, top_k), dtype=torch.float32, device=qk.device)
+    check(_lib.lib().mivos_memory_read_wide_sets(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, sets, top_k,
+                                                 _ptr(out), out.shape[-1], out_coff, hh, ww, _ptr(idx), _ptr(val),
+                                                 _ptr(workspace), workspace.numel(), _ptr(counts), _f16(out),
+                                                 _stream()),
+          "mivos_memory_read_wide_sets")
+    return (out, idx, val) if want_topk else out
+
+
+def _set_counts(who: str, qk: torch.Tensor, counts: torch.Tensor) -> int:
+    """Query sets of a per-set read: qk [sets,hw,128] and one int32 live slot count per set in `counts` (device)."""
+    _req(counts, torch.int32)
+    if qk.dim() != 3 or counts.numel() < qk.shape[0]:
+        raise _lib.MivosError(f"{who}: per-set counts need a [sets,hw,128] query tensor and one count per set")
+    return qk.shape[0]
 
 
 def upsample4x_sigmoid_aggregate(logits: torch.Tensor, k: int, h4: int, w4: int, coff: int = 0,

@@ -81,3 +81,17 @@ def bank_capacity_frames(t: int, mem_freq: int, num_certain: int, total_m: int) 
     is within the budget), so every pass and every session over clips of this length shares one entry
     of the frame-step cache."""
     return max(total_m, (t - 2) // mem_freq + 2 + INTERACTION_BUDGET)
+
+
+def pass_order(plans: List[PassPlan]) -> List[int]:
+    """Clips of one lock-step pass, longest pass first (stable on ties).  In this order the clips that still have a
+    frame at tick i are a prefix (those with more than i frames), and so are the clips that memorize at tick i: a
+    clip skips the memorize only on its last frame, so they are those with more than i + 1 frames."""
+    return sorted(range(len(plans)), key=lambda c: -len(plans[c].frames))
+
+
+def tick_prefixes(plans: List[PassPlan], order: List[int], i: int):
+    """(clips with a frame at tick i, clips memorizing at tick i), both prefixes of `order`."""
+    n = sum(1 for c in order if len(plans[c].frames) > i)
+    n_mem = sum(1 for c in order[:n] if plans[c].frames[i].memorize)
+    return n, n_mem
