@@ -298,6 +298,56 @@ MIVOS_API int mivos_memory_read_wide_sets(const float* bank_k, const float* bank
                       void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
                       int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
                       const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
+
+/* Object-group forms: lock-step clips with different object counts.  A batch of `maps` object maps (k_objects for
+ * the reads) is split into `groups` runs of consecutive maps by `first`, a DEVICE array of groups + 1 int32 entries
+ * read at run time (required): the exclusive prefix sums of the groups' object counts, so group g owns maps
+ * [first[g], first[g+1]) and first[groups] = maps.  1 <= groups <= maps.  The host cannot check the table: a map
+ * that no group inside [0, maps] holds (an empty group, a group past `maps`, a table that is not ascending) takes
+ * part in nothing and never causes a fault; a table that is not ascending may also make groups overlap, and the
+ * maps they share then get the (racing) result of either group — never a write outside the operands.  With the uniform table first = [0, K, 2K, ...] each form gives the bits
+ * of the per-set / groups / skip_n / src_n form it generalises.
+ * - the three reads: object o of group g reads query set g of qk [groups][hw][128] and the live slots
+ *   0 .. dyn_slots[g] - 1 of its own bank (one count per group); everything else as the per-set forms.  An object in
+ *   no group reads no slot.
+ * - mivos_bank_write_groups: group g writes its maps to bank frame dyn_t[g] (outside [0, t_max]: nothing).
+ * - mivos_stem_gather_s2d_groups (the memorize stem, kpad >= 80): image i, object j = i - first[g] of group g, reads
+ *   frame g (frames frame_gstride floats apart) and the PACKED planes [maps + groups, H, W] of `planes`: group g's
+ *   background plane first[g] + g, then its objects; the "others" channel sums group g's other objects only.
+ * - mivos_upsample2x_add_groups (`skip` required) / mivos_halo_copy_groups: skip / source map g is broadcast over the
+ *   images of group g (the HALO maps of n images; an image in no group is not written).
+ * - mivos_upsample4x_sigmoid_aggregate_groups: the register kernel of mivos_upsample4x_sigmoid_aggregate within each
+ *   group of at most 16 maps (maps <= 16 * groups; a larger group writes nothing): raw_out plane first[g] + j,
+ *   prob_out PACKED planes [maps + groups, 1, H, W], group g's background at first[g] + g, then its objects.       */
+MIVOS_API int mivos_memory_read_groups(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int groups, const int32_t* first,
+                      int top_k, void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
+                      int algo, const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
+MIVOS_API int mivos_memory_read_dense_groups(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int groups, const int32_t* first,
+                      void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      void* workspace, int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
+                      mivos_stream_t stream);
+MIVOS_API int mivos_memory_read_wide_groups(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                      int k_objects, int64_t slots, const float* qk, int hw, int groups, const int32_t* first,
+                      int top_k, void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
+                      int32_t* topk_idx, float* topk_val, void* workspace, int64_t workspace_bytes,
+                      const int32_t* dyn_slots, int out_f16, mivos_stream_t stream);
+MIVOS_API int mivos_bank_write_groups(const float* halo, int maps, int groups, const int32_t* first, int h, int w,
+                      int cstride, int coff_k, int coff_v, float* bank_k, float* bank_v, int64_t slots_cap,
+                      int t_max, const int32_t* dyn_t, mivos_stream_t stream);
+MIVOS_API int mivos_stem_gather_s2d_groups(const float* frame, const float* planes, int maps, int groups,
+                      const int32_t* first, int h, int w, void* out, int kpad, int out_f16, int64_t frame_gstride,
+                      mivos_stream_t stream);
+MIVOS_API int mivos_upsample2x_add_groups(void* x, const void* up, int n, int h, int w, int c, void* x_relu,
+                      const void* skip, int groups, const int32_t* first, int f16, mivos_stream_t stream);
+MIVOS_API int mivos_halo_copy_groups(const void* src, int groups, const int32_t* first, int src_cstride,
+                      int src_coff, void* dst, int dst_cstride, int dst_coff, int n, int h, int w, int c, int relu,
+                      int src_f16, int dst_f16, mivos_stream_t stream);
+MIVOS_API int mivos_upsample4x_sigmoid_aggregate_groups(const float* logits, int maps, int groups,
+                      const int32_t* first, int h4, int w4, int cstride, int coff, float* raw_out, float* prob_out,
+                      mivos_stream_t stream);
 /* Diagnostic, synchronising: candidate statistics of the last tensor-core-path read in `workspace`:
  * out[0] total candidates, out[1] max per (object, query), out[2] queries served by the exact
  * fallback, out[3] splits of the memory axis.                                                    */

@@ -90,6 +90,14 @@ SIGNATURES = {
     "mivos_memory_read_sets": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _i, _p, _i, _p]),
     "mivos_memory_read_dense_sets": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _i, _i, _i, _p, _l, _p, _i, _p]),
     "mivos_memory_read_wide_sets": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _p, _i, _p]),
+    "mivos_memory_read_groups": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _i, _p, _i, _p]),
+    "mivos_memory_read_dense_groups": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _p, _i, _i, _i, _i, _p, _l, _p, _i, _p]),
+    "mivos_memory_read_wide_groups": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _p, _i, _i, _i, _i, _p, _p, _p, _l, _p, _i, _p]),
+    "mivos_bank_write_groups": (_i, [_p, _i, _i, _p, _i, _i, _i, _i, _i, _p, _p, _l, _i, _p, _p]),
+    "mivos_stem_gather_s2d_groups": (_i, [_p, _p, _i, _i, _p, _i, _i, _p, _i, _i, _l, _p]),
+    "mivos_upsample2x_add_groups": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _p, _i, _p]),
+    "mivos_halo_copy_groups": (_i, [_p, _i, _p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
+    "mivos_upsample4x_sigmoid_aggregate_groups": (_i, [_p, _i, _i, _p, _i, _i, _i, _i, _p, _p, _p]),
     "mivos_memory_read_stats": (_i, [_p, _i, _l, _i, _i, C.POINTER(_l)]),
     "mivos_memory_read_dense_workspace": (_l, [_i, _l, _i]),
     "mivos_memory_read_dense": (_i, [_p, _p, _l, _i, _l, _p, _i, _i, _p, _i, _i, _i, _i, _p, _l, _p, _i, _p]),

@@ -2,6 +2,7 @@
 // bilinear resampling, layout conversion at the API boundary, soft aggregation and argmax.
 // All are coalesced / 128-bit vectorised streaming kernels; none has data reuse worth staging
 // beyond the transposes (which go through a padded shared-memory tile).
+#include "groups.cuh"
 #include "host_util.h"
 #include "pdl.cuh"
 
@@ -30,12 +31,14 @@ __device__ __forceinline__ void bilin(int dst, float scale, int in_size, int& i0
 }
 
 // ------------------------------------------------------------------------------------------
-// SETS: set s (per_set consecutive objects) writes bank frame dyn_t[s]; a frame outside [0, t] writes nothing
-template <bool SETS>
+// SETS: set s (per_set consecutive objects) writes bank frame dyn_t[s]; a frame outside [0, t] writes nothing.
+// GROUPS (with SETS): the set of an object is its group in `first` (groups.cuh); an object in no group writes nothing.
+template <bool SETS, bool GROUPS = false>
 __global__ void bank_write_kernel(const float4* __restrict__ halo, int kobj, int h, int w,
                                   int cstride4, int coffk4, int coffv4, float4* __restrict__ bank_k,
                                   float4* __restrict__ bank_v, int64_t slots_cap, int t,
-                                  const int* __restrict__ dyn_t, int per_set) {
+                                  const int* __restrict__ dyn_t, int per_set, const int* __restrict__ first,
+                                  int groups) {
   mivos::pdl_prologue();
   const int t_max = t;
   if (!SETS && dyn_t) t = *dyn_t;  // bank slot from device memory (CUDA-graph replay)
@@ -49,7 +52,9 @@ __global__ void bank_write_kernel(const float4* __restrict__ halo, int kobj, int
     const int p = static_cast<int>(t1 % hw);
     const int obj = static_cast<int>(t1 / hw);
     if (SETS) {
-      t = dyn_t[obj / per_set];
+      const int s = GROUPS ? map_group(first, groups, kobj, obj) : obj / per_set;
+      if (GROUPS && s < 0) continue;
+      t = dyn_t[s];
       if (t < 0 || t > t_max) continue;
     }
     const int y = p / w, x = p - y * w;
@@ -114,10 +119,15 @@ __device__ __forceinline__ void aggregate_pixel(const float* p, int k, bool hard
   for (int j = 0; j <= k; ++j) o[j] = o[j] / s;
 }
 
+// GROUPS: group g is maps [first[g], first[g+1]) of `kobj` maps (groups.cuh), its planes start at first[g] in
+// raw_out and at first[g] + g in prob_out (packed: each group's background plane, then its objects); a group that is
+// empty, outside [0, kobj] or of more than kMaxObjects maps writes nothing.
+template <bool GROUPS>
 __global__ void upsample4x_sigmoid_aggregate_kernel(const float* __restrict__ logits_all, int kobj,
                                                     int h4, int w4, int cstride, int coff,
                                                     float* __restrict__ raw_all,
-                                                    float* __restrict__ prob_all, int groups) {
+                                                    float* __restrict__ prob_all, int groups,
+                                                    const int* __restrict__ first) {
   mivos::pdl_prologue();
   const int H = 4 * h4, W = 4 * w4;
   const int64_t plane = static_cast<int64_t>(H) * W;
@@ -127,9 +137,12 @@ __global__ void upsample4x_sigmoid_aggregate_kernel(const float* __restrict__ lo
        ig += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int g = static_cast<int>(ig / plane);
     const int64_t i = ig - static_cast<int64_t>(g) * plane;
-    const float* logits = logits_all + static_cast<int64_t>(g) * kobj * (h4 + 2) * (w4 + 2) * cstride;
-    float* raw_out = raw_all ? raw_all + static_cast<int64_t>(g) * kobj * plane : nullptr;
-    float* prob_out = prob_all ? prob_all + static_cast<int64_t>(g) * (kobj + 1) * plane : nullptr;
+    int m0 = g * kobj, k = kobj;
+    if (GROUPS && (!group_range(first, kobj, g, &m0, &k) || k > kMaxObjects)) continue;
+    const int64_t p0 = GROUPS ? m0 + g : static_cast<int64_t>(g) * (kobj + 1);
+    const float* logits = logits_all + static_cast<int64_t>(m0) * (h4 + 2) * (w4 + 2) * cstride;
+    float* raw_out = raw_all ? raw_all + static_cast<int64_t>(m0) * plane : nullptr;
+    float* prob_out = prob_all ? prob_all + p0 * plane : nullptr;
     const int y = static_cast<int>(i / W), x = static_cast<int>(i - static_cast<int64_t>(y) * W);
     int y0, y1, x0, x1;
     float ly, lx;
@@ -137,7 +150,7 @@ __global__ void upsample4x_sigmoid_aggregate_kernel(const float* __restrict__ lo
     bilin(x, 0.25f, w4, x0, x1, lx);
     const float hy = 1.f - ly, hx = 1.f - lx;
     float p[kMaxObjects], o[kMaxObjects + 1];
-    for (int j = 0; j < kobj; ++j) {
+    for (int j = 0; j < k; ++j) {
       const int64_t base = static_cast<int64_t>(j) * (h4 + 2);
       const float v00 = logits[((base + y0 + 1) * (w4 + 2) + x0 + 1) * cstride + coff];
       const float v01 = logits[((base + y0 + 1) * (w4 + 2) + x1 + 1) * cstride + coff];
@@ -148,8 +161,8 @@ __global__ void upsample4x_sigmoid_aggregate_kernel(const float* __restrict__ lo
       if (raw_out) raw_out[j * plane + i] = p[j];
     }
     if (prob_out) {
-      aggregate_pixel(p, kobj, false, o);
-      for (int j = 0; j <= kobj; ++j) prob_out[j * plane + i] = o[j];
+      aggregate_pixel(p, k, false, o);
+      for (int j = 0; j <= k; ++j) prob_out[j * plane + i] = o[j];
     }
   }
 }
@@ -481,7 +494,7 @@ extern "C" MIVOS_API int mivos_bank_write(const float* halo, int k_objects, int 
   const int64_t total = static_cast<int64_t>(k_objects) * h * w * 160;
   launch_pdl(bank_write_kernel<false>, capped_grid(total), kThreads, 0, ST(s), 
       reinterpret_cast<const float4*>(halo), k_objects, h, w, cstride / 4, coff_k / 4, coff_v / 4,
-      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t, dyn_t, 0);
+      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t, dyn_t, 0, nullptr, 0);
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }
@@ -500,7 +513,29 @@ extern "C" MIVOS_API int mivos_bank_write_sets(const float* halo, int k_objects,
   const int64_t total = static_cast<int64_t>(k_objects) * h * w * 160;
   launch_pdl(bank_write_kernel<true>, capped_grid(total), kThreads, 0, ST(s),
       reinterpret_cast<const float4*>(halo), k_objects, h, w, cstride / 4, coff_k / 4, coff_v / 4,
-      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t_max, dyn_t, k_objects / sets);
+      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t_max, dyn_t, k_objects / sets,
+      nullptr, 0);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_bank_write_groups(const float* halo, int maps, int groups, const int32_t* first, int h,
+                                                 int w, int cstride, int coff_k, int coff_v, float* bank_k,
+                                                 float* bank_v, int64_t slots_cap, int t_max, const int32_t* dyn_t,
+                                                 mivos_stream_t s) {
+  MIVOS_REQUIRE(dyn_t, "bank_write_groups: null frame array (one device-side bank frame per group)");
+  MIVOS_REQUIRE(first, "bank_write_groups: null group table (groups + 1 device-side first maps)");
+  MIVOS_REQUIRE(groups >= 1 && groups <= maps, "bank_write_groups: %d groups for %d maps (1 <= groups <= maps)", groups,
+                maps);
+  MIVOS_REQUIRE(halo && bank_k && bank_v && AL16(halo) && AL16(bank_k) && AL16(bank_v),
+                "bank_write_groups: null/unaligned pointer");
+  MIVOS_REQUIRE(cstride % 4 == 0 && coff_k % 4 == 0 && coff_v % 4 == 0 && t_max >= 0 &&
+                    static_cast<int64_t>(t_max + 1) * h * w <= slots_cap,
+                "bank_write_groups: slot %d does not fit capacity %lld", t_max, (long long)slots_cap);
+  const int64_t total = static_cast<int64_t>(maps) * h * w * 160;
+  launch_pdl(bank_write_kernel<true, true>, capped_grid(total), kThreads, 0, ST(s),
+      reinterpret_cast<const float4*>(halo), maps, h, w, cstride / 4, coff_k / 4, coff_v / 4,
+      reinterpret_cast<float4*>(bank_k), reinterpret_cast<float4*>(bank_v), slots_cap, t_max, dyn_t, 0, first, groups);
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }
@@ -529,8 +564,26 @@ extern "C" MIVOS_API int mivos_upsample4x_sigmoid_aggregate(const float* logits,
   MIVOS_REQUIRE(k_objects >= 1 && k_objects <= kMaxObjects, "upsample4x: %d objects (max %d)", k_objects, kMaxObjects);
   MIVOS_REQUIRE(groups >= 1, "upsample4x: groups must be >= 1");
   const int64_t plane = 16ll * h4 * w4;
-  launch_pdl(upsample4x_sigmoid_aggregate_kernel, capped_grid(plane * groups), kThreads, 0, ST(s), 
-      logits, k_objects, h4, w4, cstride, coff, raw_out, prob_out, groups);
+  launch_pdl(upsample4x_sigmoid_aggregate_kernel<false>, capped_grid(plane * groups), kThreads, 0, ST(s), 
+      logits, k_objects, h4, w4, cstride, coff, raw_out, prob_out, groups, nullptr);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_upsample4x_sigmoid_aggregate_groups(const float* logits, int maps, int groups,
+                                                                   const int32_t* first, int h4, int w4, int cstride,
+                                                                   int coff, float* raw_out, float* prob_out,
+                                                                   mivos_stream_t s) {
+  MIVOS_REQUIRE(first, "upsample4x_groups: null group table (groups + 1 device-side first maps)");
+  MIVOS_REQUIRE(logits && (raw_out || prob_out), "upsample4x_groups: null pointer");
+  MIVOS_REQUIRE(groups >= 1 && groups <= maps, "upsample4x_groups: %d groups for %d maps (1 <= groups <= maps)", groups,
+                maps);
+  MIVOS_REQUIRE(maps <= kMaxObjects * groups, "upsample4x_groups: %d maps in %d groups (max %d objects per group)", maps,
+                groups, kMaxObjects);
+  MIVOS_REQUIRE(h4 >= 1 && w4 >= 1 && coff >= 0 && coff < cstride, "upsample4x_groups: bad shape");
+  const int64_t plane = 16ll * h4 * w4;
+  launch_pdl(upsample4x_sigmoid_aggregate_kernel<true>, capped_grid(plane * groups), kThreads, 0, ST(s), logits, maps,
+             h4, w4, cstride, coff, raw_out, prob_out, groups, first);
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }

@@ -3,6 +3,7 @@
 // All are HBM-bound streaming kernels working on 16-byte vectors (4 x fp32 / 8 x fp16) with the
 // channel index fastest, so every warp access is a run of full 128-byte lines; arithmetic is done
 // in fp32 and rounded to nearest-even on store.
+#include "groups.cuh"
 #include "host_util.h"
 #include "pdl.cuh"
 
@@ -203,11 +204,14 @@ cudaError_t reserve_stem_smem(int smem) {
 // element type with 4 pixels of zero padding on each side (the "others" channel of the memorize stem is
 // formed here), so a matrix row is two contiguous runs of 8*CIN staged values; a thread assembles one
 // 16-byte piece, a warp writes 512 contiguous bytes.
-template <int CIN, typename T>
+// GROUPS (mask form): image i is object i - first[g] of the group g that holds it (groups.cuh; `kobj` = all maps),
+// which reads frame g and its objects' planes first[g] + g + 1 + j of the packed planes `masks` (each group's
+// background plane, then its objects); "others" sums over group g only.  An image in no group writes nothing.
+template <int CIN, typename T, bool GROUPS = false>
 __global__ void __launch_bounds__(256)
 stem_s2d_gather_kernel(const float* __restrict__ frame, const float* __restrict__ masks, int kobj, int h, int w,
                        T* __restrict__ out, int kpad, int64_t frame_gstride, int64_t mask_gstride, int obj0,
-                       int nobj) {
+                       int nobj, const int* __restrict__ first, int groups) {
   mivos::pdl_prologue();
   extern __shared__ __align__(16) uint8_t s2d_smem[];
   T* rowbuf = reinterpret_cast<T*>(s2d_smem);  // [2][w + 8][CIN]
@@ -216,12 +220,20 @@ stem_s2d_gather_kernel(const float* __restrict__ frame, const float* __restrict_
   const int yo = static_cast<int>(blockIdx.x) - 1;  // output row; -1 and ho are border rows (zeros)
   const int img = blockIdx.y;
   // the mask form gathers objects [obj0, obj0 + nobj) of each group of kobj (all of them but in object-chunked memorize)
-  const int obj = CIN == 5 ? obj0 + img % nobj : img;
-  if constexpr (CIN == 5) {
+  int obj = CIN == 5 ? obj0 + img % nobj : img;
+  const int64_t plane = static_cast<int64_t>(h) * w;
+  if constexpr (GROUPS) {
+    const int g = map_group(first, groups, kobj, img);
+    if (g < 0) return;  // the whole CTA: no barrier has been reached
+    int m0;
+    group_range(first, kobj, g, &m0, &kobj);
+    obj = img - m0;
+    frame += static_cast<int64_t>(g) * frame_gstride;
+    masks += (static_cast<int64_t>(m0) + g + 1) * plane;
+  } else if constexpr (CIN == 5) {
     frame += static_cast<int64_t>(img / nobj) * frame_gstride;
     masks += static_cast<int64_t>(img / nobj) * mask_gstride;
   }
-  const int64_t plane = static_cast<int64_t>(h) * w;
   const int rowlen = (w + 8) * CIN;
   const bool live_row = yo >= 0 && yo < ho;
   if (live_row) {
@@ -353,9 +365,11 @@ __device__ __forceinline__ void bilin(int dst, float scale, int in_size, int& i0
   l1 = src - static_cast<float>(i0);
 }
 
-template <typename T>
+// GROUPS: skip map g serves the images of group g of `first` (groups.cuh); an image in no group is left as it is
+template <typename T, bool GROUPS = false>
 __global__ void upsample2x_add_kernel(T* __restrict__ x, const T* __restrict__ up, int n, int h, int w, int cv,
-                                      T* __restrict__ x_relu, const T* __restrict__ skip, int per_skip) {
+                                      T* __restrict__ x_relu, const T* __restrict__ skip, int per_skip,
+                                      const int* __restrict__ first, int groups) {
   mivos::pdl_prologue();
   constexpr int N = V16<T>::N;
   const int hs = h / 2, ws = w / 2;
@@ -368,6 +382,11 @@ __global__ void upsample2x_add_kernel(T* __restrict__ x, const T* __restrict__ u
     t1 /= w;
     const int yo = static_cast<int>(t1 % h);
     const int img = static_cast<int>(t1 / h);
+    int simg = 0;
+    if constexpr (GROUPS) {
+      simg = map_group(first, groups, n, img);
+      if (simg < 0) continue;
+    }
     int y0, y1, x0, x1;
     float ly, lx;
     bilin(yo, 0.5f, hs, y0, y1, ly);
@@ -382,7 +401,8 @@ __global__ void upsample2x_add_kernel(T* __restrict__ x, const T* __restrict__ u
     const int64_t o = (((static_cast<int64_t>(img) * (h + 2) + yo + 1) * (w + 2) + xo + 1) * cv + ci) * N;
     // `skip` (one map per `per_skip` consecutive images: a frame's skip path broadcast over its objects)
     // replaces x as the addend: x = skip + up2x(up)
-    if (skip) V16<T>::load(skip + (((static_cast<int64_t>(img / per_skip) * (h + 2) + yo + 1) * (w + 2) + xo + 1) * cv + ci) * N, xv);
+    if (GROUPS) V16<T>::load(skip + (((static_cast<int64_t>(simg) * (h + 2) + yo + 1) * (w + 2) + xo + 1) * cv + ci) * N, xv);
+    else if (skip) V16<T>::load(skip + (((static_cast<int64_t>(img / per_skip) * (h + 2) + yo + 1) * (w + 2) + xo + 1) * cv + ci) * N, xv);
     else V16<T>::load(x + o, xv);
     float r[N];
 #pragma unroll
@@ -398,9 +418,12 @@ __global__ void upsample2x_add_kernel(T* __restrict__ x, const T* __restrict__ u
 
 // ------------------------------------------------------------------------------------------
 // channel-window copy between HALO maps with optional ReLU and type conversion; 4 channels/thread
-template <typename TS, typename TD>
+// GROUPS: source map g serves the images of group g of `first` (src_n groups, groups.cuh); an image in no group is
+// not written
+template <typename TS, typename TD, bool GROUPS = false>
 __global__ void halo_copy_kernel(const TS* __restrict__ src, int src_n, int src_cs, int src_co, TD* __restrict__ dst,
-                                 int dst_cs, int dst_co, int n, int h, int w, int c4, int relu) {
+                                 int dst_cs, int dst_co, int n, int h, int w, int c4, int relu,
+                                 const int* __restrict__ first) {
   mivos::pdl_prologue();
   const int64_t total = static_cast<int64_t>(n) * h * w * c4;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < total;
@@ -411,7 +434,9 @@ __global__ void halo_copy_kernel(const TS* __restrict__ src, int src_n, int src_
     t1 /= w;
     const int y = static_cast<int>(t1 % h);
     const int img = static_cast<int>(t1 / h);
-    const int simg = img / (n / src_n);  // src_n maps broadcast over n / src_n consecutive images each
+    // src_n maps broadcast over n / src_n consecutive images each, or over the images of their group
+    const int simg = GROUPS ? map_group(first, src_n, n, img) : img / (n / src_n);
+    if (GROUPS && simg < 0) continue;
     const int64_t rs = (static_cast<int64_t>(simg) * (h + 2) + y + 1) * (w + 2) + x + 1;
     const int64_t rd = (static_cast<int64_t>(img) * (h + 2) + y + 1) * (w + 2) + x + 1;
     const TS* s = src + rs * src_cs + src_co + ci * 4;
@@ -685,7 +710,7 @@ int stem_s2d(const char* who, const float* frame, const float* masks, int k_obje
       configured = smem;                                                                                   \
     }                                                                                                      \
     launch_pdl(stem_s2d_gather_kernel<CIN_, T_>, grid, 256, smem, ST(s), frame, masks, k_objects, h, w,    \
-               static_cast<T_*>(out), kpad, frame_gstride, mask_gstride, obj0, nobj);                      \
+               static_cast<T_*>(out), kpad, frame_gstride, mask_gstride, obj0, nobj, nullptr, 0);         \
   } while (0)
   if (out_f16) {
     if (masks) S2D(5, __half);
@@ -708,6 +733,38 @@ extern "C" MIVOS_API int mivos_stem_gather_s2d(const float* frame, const float* 
   MIVOS_REQUIRE(h % 2 == 0 && w % 2 == 0 && h > 0 && w > 0 && k_objects >= 1, "stem_gather_s2d: h,w must be even");
   return stem_s2d("stem_gather_s2d", frame, masks, k_objects, 0, k_objects, h, w, out, kpad, out_f16, groups,
                   frame_gstride, mask_gstride, s);
+}
+
+extern "C" MIVOS_API int mivos_stem_gather_s2d_groups(const float* frame, const float* planes, int maps, int groups,
+                                                      const int32_t* first, int h, int w, void* out, int kpad,
+                                                      int out_f16, int64_t frame_gstride, mivos_stream_t s) {
+  MIVOS_REQUIRE(first, "stem_gather_s2d_groups: null group table (groups + 1 device-side first maps)");
+  MIVOS_REQUIRE(frame && planes && out, "stem_gather_s2d_groups: null pointer");
+  MIVOS_REQUIRE(groups >= 1 && groups <= maps && maps <= 65535,
+                "stem_gather_s2d_groups: %d groups for %d maps (1 <= groups <= maps)", groups, maps);
+  MIVOS_REQUIRE(h % 2 == 0 && w % 2 == 0 && h > 0 && w > 0, "stem_gather_s2d_groups: h,w must be even");
+  const int v = out_f16 ? 8 : 4;
+  MIVOS_REQUIRE(kpad >= 16 * 5 && kpad % v == 0 && AL16(out), "stem_gather_s2d_groups: kpad %d too small / unaligned",
+                kpad);
+  const dim3 grid(h / 2 + 2, maps);
+  const int smem = 2 * (w + 8) * 5 * (out_f16 ? 2 : 4);
+  MIVOS_REQUIRE(smem <= 227 * 1024, "stem_gather_s2d_groups: a %d-pixel wide frame needs %d B of shared memory", w, smem);
+#define S2DG(T_)                                                                                           \
+  do {                                                                                                     \
+    static int configured = 48 * 1024;                                                                     \
+    if (smem > configured) {                                                                               \
+      MIVOS_CUDA_OK(cudaFuncSetAttribute(stem_s2d_gather_kernel<5, T_, true>,                              \
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem));              \
+      configured = smem;                                                                                   \
+    }                                                                                                      \
+    launch_pdl(stem_s2d_gather_kernel<5, T_, true>, grid, 256, smem, ST(s), frame, planes, maps, h, w,     \
+               static_cast<T_*>(out), kpad, frame_gstride, int64_t{0}, 0, maps, first, groups);            \
+  } while (0)
+  if (out_f16) S2DG(__half);
+  else S2DG(float);
+#undef S2DG
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
 }
 
 extern "C" MIVOS_API int mivos_stem_gather_s2d_range(const float* frame, const float* masks, int k_objects, int obj0,
@@ -863,11 +920,34 @@ extern "C" MIVOS_API int mivos_upsample2x_add(void* x, const void* up, int n, in
   if (f16)
     launch_pdl(upsample2x_add_kernel<__half>, capped_grid(total), kThreads, 0, ST(s), 
         static_cast<__half*>(x), static_cast<const __half*>(up), n, h, w, c / v, static_cast<__half*>(x_relu),
-        static_cast<const __half*>(skip), per_skip);
+        static_cast<const __half*>(skip), per_skip, nullptr, 0);
   else
     launch_pdl(upsample2x_add_kernel<float>, capped_grid(total), kThreads, 0, ST(s), 
         static_cast<float*>(x), static_cast<const float*>(up), n, h, w, c / v, static_cast<float*>(x_relu),
-        static_cast<const float*>(skip), per_skip);
+        static_cast<const float*>(skip), per_skip, nullptr, 0);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_upsample2x_add_groups(void* x, const void* up, int n, int h, int w, int c, void* x_relu,
+                                                     const void* skip, int groups, const int32_t* first, int f16,
+                                                     mivos_stream_t s) {
+  const int v = f16 ? 8 : 4;
+  MIVOS_REQUIRE(first, "upsample2x_add_groups: null group table (groups + 1 device-side first maps)");
+  MIVOS_REQUIRE(x && up && skip && AL16(x) && AL16(up) && (!x_relu || AL16(x_relu)) && AL16(skip) && c % v == 0 &&
+                    h % 2 == 0 && w % 2 == 0,
+                "upsample2x_add_groups: bad arguments");
+  MIVOS_REQUIRE(groups >= 1 && groups <= n, "upsample2x_add_groups: %d groups for %d images (1 <= groups <= images)",
+                groups, n);
+  const int64_t total = static_cast<int64_t>(n) * h * w * (c / v);
+  if (f16)
+    launch_pdl(upsample2x_add_kernel<__half, true>, capped_grid(total), kThreads, 0, ST(s), static_cast<__half*>(x),
+               static_cast<const __half*>(up), n, h, w, c / v, static_cast<__half*>(x_relu),
+               static_cast<const __half*>(skip), 0, first, groups);
+  else
+    launch_pdl(upsample2x_add_kernel<float, true>, capped_grid(total), kThreads, 0, ST(s), static_cast<float*>(x),
+               static_cast<const float*>(up), n, h, w, c / v, static_cast<float*>(x_relu),
+               static_cast<const float*>(skip), 0, first, groups);
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }
@@ -882,12 +962,35 @@ extern "C" MIVOS_API int mivos_halo_copy(const void* src, int src_n, int src_cst
   const unsigned g = capped_grid(total);
 #define HC(TS, TD)                                                                                              \
   launch_pdl(halo_copy_kernel<TS, TD>, g, kThreads, 0, ST(s), static_cast<const TS*>(src), src_n, src_cstride, src_coff, \
-                                                      static_cast<TD*>(dst), dst_cstride, dst_coff, n, h, w, c / 4, relu)
+                                                      static_cast<TD*>(dst), dst_cstride, dst_coff, n, h, w, c / 4, relu, nullptr)
   if (src_f16 && dst_f16) HC(__half, __half);
   else if (src_f16) HC(__half, float);
   else if (dst_f16) HC(float, __half);
   else HC(float, float);
 #undef HC
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_halo_copy_groups(const void* src, int groups, const int32_t* first, int src_cstride,
+                                                int src_coff, void* dst, int dst_cstride, int dst_coff, int n, int h,
+                                                int w, int c, int relu, int src_f16, int dst_f16, mivos_stream_t s) {
+  MIVOS_REQUIRE(first, "halo_copy_groups: null group table (groups + 1 device-side first maps)");
+  MIVOS_REQUIRE(src && dst, "halo_copy_groups: null pointer");
+  MIVOS_REQUIRE(groups >= 1 && groups <= n, "halo_copy_groups: %d groups for %d images (1 <= groups <= images)", groups,
+                n);
+  MIVOS_REQUIRE(c % 4 == 0 && src_coff + c <= src_cstride && dst_coff + c <= dst_cstride,
+                "halo_copy_groups: bad channel window");
+  const int64_t total = static_cast<int64_t>(n) * h * w * (c / 4);
+  const unsigned g = capped_grid(total);
+#define HCG(TS, TD)                                                                                               \
+  launch_pdl(halo_copy_kernel<TS, TD, true>, g, kThreads, 0, ST(s), static_cast<const TS*>(src), groups, src_cstride, \
+             src_coff, static_cast<TD*>(dst), dst_cstride, dst_coff, n, h, w, c / 4, relu, first)
+  if (src_f16 && dst_f16) HCG(__half, __half);
+  else if (src_f16) HCG(__half, float);
+  else if (dst_f16) HCG(float, __half);
+  else HCG(float, float);
+#undef HCG
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }

@@ -84,7 +84,8 @@ memread_exact_kernel(const float* __restrict__ bank_k, int64_t slots_cap, int64_
                      const float* __restrict__ qk_all, int hw, int q_div, int top_k, int tiles_per_split,
                      int splits, int2* __restrict__ cand,
                      int* __restrict__ cand_cnt, const int* __restrict__ flags,
-                     const int* __restrict__ dyn_slots, int dyn_set_stride) {
+                     const int* __restrict__ dyn_slots, int dyn_set_stride, const int* __restrict__ first,
+                     int groups) {
   mivos::pdl_prologue();
   extern __shared__ __align__(16) uint8_t smem_raw[];
   A1Smem& sm = *reinterpret_cast<A1Smem*>(smem_raw);
@@ -97,7 +98,9 @@ memread_exact_kernel(const float* __restrict__ bank_k, int64_t slots_cap, int64_
     if (!__syncthreads_or(mine)) return;
   }
   const float* keys = bank_k + static_cast<int64_t>(obj) * slots_cap * 128;
-  const float* qk = qk_all + static_cast<int64_t>(q_div > 0 ? obj / q_div : 0) * hw * 128;  // this object's query set
+  // this object's query set (object groups: -1 for an object in no group, which reads set 0 over no slot)
+  const int qset = first ? map_group(first, groups, gridDim.z, obj) : (q_div > 0 ? obj / q_div : 0);
+  const float* qk = qk_all + static_cast<int64_t>(qset < 0 ? 0 : qset) * hw * 128;
 
   // queries, pre-divided by sqrt(CK) (prop_net.py:86)
   for (int i = tid; i < A1_Q * 128; i += A1_THREADS) {
@@ -110,7 +113,7 @@ memread_exact_kernel(const float* __restrict__ bank_k, int64_t slots_cap, int64_
   }
   __syncthreads();
 
-  slots = live_slots(dyn_slots, slots, slots_cap, q_div > 0 ? obj / q_div : 0, dyn_set_stride);
+  slots = qset < 0 ? 0 : live_slots(dyn_slots, slots, slots_cap, qset, dyn_set_stride);
   if (dyn_slots) {  // device-side slot count (CUDA-graph replay): fixed grid, ranges derived here
     const int tiles = static_cast<int>((slots + A1_S - 1) / A1_S);
     tiles_per_split = (tiles + splits - 1) / splits;
@@ -247,7 +250,7 @@ memread_select_kernel(const MemreadArgs a, const int top_k, const SelectLists L,
   const int hw = a.hw;
   if (lq >= static_cast<int64_t>(a.k_objects) * hw) return;
   const int obj = static_cast<int>(lq / hw), q = static_cast<int>(lq - static_cast<int64_t>(obj) * hw);
-  const int qset = a.q_div > 0 ? obj / a.q_div : 0;  // query set of this object (lock-step clips: one per clip)
+  const int qset = query_set(a, obj);  // query set of this object (lock-step clips: one per clip)
   uint8_t* wb = sel_smem + warp * ((kSelBytesPerWarp + 15) & ~15);
   float* cs = reinterpret_cast<float*>(wb);          // [B_MAXSURV] candidate scores
   int* ci = reinterpret_cast<int*>(cs + B_MAXSURV);  // [B_MAXSURV] candidate slots
@@ -491,7 +494,8 @@ int launch_exact_candidates(const MemreadArgs& a, int top_k, const MemreadPlan& 
   dim3 grid(pl.qtiles, pl.splits, a.k_objects);
   launch_pdl(memread_exact_kernel, grid, A1_THREADS, sizeof(A1Smem), stream, a.bank_k, a.slots_cap, a.slots, a.qk, a.hw,
              a.q_div, top_k, pl.tiles_per_split, pl.splits, reinterpret_cast<int2*>(plan_lists(w, pl)),
-             reinterpret_cast<int*>(w + pl.off_cnt), flags, a.dyn_slots, a.dyn_set_stride);
+             reinterpret_cast<int*>(w + pl.off_cnt), flags, a.dyn_slots, a.dyn_set_stride, a.first,
+             a.groups);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
   return MIVOS_OK;
@@ -538,6 +542,18 @@ int memread_sets_args(MemreadArgs& a, int sets, const char* who) {
                 "%s: %d sets do not divide %d objects", who, sets, a.k_objects);
   a.q_div = a.k_objects / sets;
   a.dyn_set_stride = 1;
+  return MIVOS_OK;
+}
+
+int memread_groups_args(MemreadArgs& a, int groups, const int* first, const char* who) {
+  MIVOS_REQUIRE(a.dyn_slots, "%s: null count array (one device-side live slot count per group)", who);
+  MIVOS_REQUIRE(first, "%s: null group table (groups + 1 device-side first objects)", who);
+  MIVOS_REQUIRE(groups >= 1 && groups <= a.k_objects, "%s: %d groups for %d objects (1 <= groups <= objects)", who,
+                groups, a.k_objects);
+  a.q_div = 0;
+  a.dyn_set_stride = 1;
+  a.first = first;
+  a.groups = groups;
   return MIVOS_OK;
 }
 
@@ -615,6 +631,21 @@ extern "C" MIVOS_API int mivos_memory_read_sets(const float* bank_k, const float
                 out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
   int rc = memread_sets_args(a, sets, "memory_read_sets");
   if (rc == MIVOS_OK) rc = memread_check_args(a, "memory_read_sets");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes, algo,
+                         reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" MIVOS_API int mivos_memory_read_groups(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                  int k_objects, int64_t slots, const float* qk, int hw, int groups,
+                                                  const int32_t* first, int top_k, void* out, int out_cstride,
+                                                  int out_coff, int out_halo_h, int out_halo_w, int32_t* topk_idx,
+                                                  float* topk_val, void* workspace, int64_t workspace_bytes, int algo,
+                                                  const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
+  MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, 0,
+                out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  int rc = memread_check_args(a, "memory_read_groups");
+  if (rc == MIVOS_OK) rc = memread_groups_args(a, groups, first, "memory_read_groups");
   if (rc != MIVOS_OK) return rc;
   return memory_read_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes, algo,
                          reinterpret_cast<cudaStream_t>(stream_));

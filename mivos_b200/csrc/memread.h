@@ -2,6 +2,7 @@
 // memread_wide.cu):
 // the operands of a read, the workspace layout of the top-k read, and the device pieces the kernels share.
 #pragma once
+#include "groups.cuh"
 #include "host_util.h"
 
 #include <cuda_fp16.h>
@@ -41,8 +42,11 @@ struct MemreadArgs {
   void* out;
   int out_cstride, out_coff, halo_h, halo_w, out_f16;
   // per-set counts (the *_sets entry points): query set s reads dyn_slots[s * dyn_set_stride]; 0: one count for all
-  // (this field fills the struct's tail padding, so the kernels' parameter blocks keep their size)
   int dyn_set_stride;
+  // object groups (the *_groups entry points): object o reads query set g and count dyn_slots[g] of the group g that
+  // holds it (groups.cuh, `groups` + 1 device entries); null: the q_div / stride mapping above
+  const int* first;
+  int groups;
 };
 
 // The operand checks both entry points share; `who` prefixes the error text.  MIVOS_OK or MIVOS_ERR_INVALID.
@@ -50,6 +54,9 @@ int memread_check_args(const MemreadArgs& a, const char* who);
 // The per-set form's extra checks (counts given, `sets` divides the objects); sets q_div = objects per set and the
 // count stride.  MIVOS_OK or MIVOS_ERR_INVALID.
 int memread_sets_args(MemreadArgs& a, int sets, const char* who);
+// The grouped form's extra checks (counts and table given, 1 <= groups <= objects); sets the group table and the
+// count stride.  MIVOS_OK or MIVOS_ERR_INVALID.
+int memread_groups_args(MemreadArgs& a, int groups, const int* first, const char* who);
 
 struct MemreadPlan {
   int algo;
@@ -113,10 +120,19 @@ __device__ __forceinline__ int64_t live_slots(const int* dyn_slots, int64_t slot
   const int64_t n = dyn_slots ? static_cast<int64_t>(dyn_slots[set * set_stride]) : slots;
   return n < slots_cap ? n : slots_cap;
 }
-// query set of object `obj`
-__device__ __forceinline__ int query_set(const MemreadArgs& a, int obj) { return a.q_div > 0 ? obj / a.q_div : 0; }
+// Query set of object `obj` and its live slots.  An object in no group (a malformed group table) reads query set 0
+// over no live slot: it takes part in no other object's read and reads no bank slot.
+__device__ __forceinline__ int object_group(const MemreadArgs& a, int obj) {
+  if (a.first) return map_group(a.first, a.groups, a.k_objects, obj);
+  return a.q_div > 0 ? obj / a.q_div : 0;
+}
+__device__ __forceinline__ int query_set(const MemreadArgs& a, int obj) {
+  const int g = object_group(a, obj);
+  return g < 0 ? 0 : g;
+}
 __device__ __forceinline__ int64_t live_slots(const MemreadArgs& a, int obj) {
-  return live_slots(a.dyn_slots, a.slots, a.slots_cap, query_set(a, obj), a.dyn_set_stride);
+  const int g = object_group(a, obj);
+  return g < 0 ? 0 : live_slots(a.dyn_slots, a.slots, a.slots_cap, g, a.dyn_set_stride);
 }
 
 // The exact score of one key row against a scaled query (q / sqrt(128)): fmaf in ascending channel order.  Every

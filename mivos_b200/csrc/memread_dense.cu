@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(D_THREADS, 1) memread_dense_kernel(const Dense
   load_tile(0, t_begin);
 
   // query tile, divided by sqrt(128) with the IEEE division of the reference (rows past hw are zero)
-  const float* qk = p.a.qk + static_cast<int64_t>(p.a.q_div > 0 ? obj / p.a.q_div : 0) * p.a.hw * 128;
+  const float* qk = p.a.qk + static_cast<int64_t>(query_set(p.a, obj)) * p.a.hw * 128;
   for (int i = tid; i < DQ * 32; i += D_THREADS) {
     const int r = i >> 5, c4 = i & 31;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -399,6 +399,20 @@ extern "C" MIVOS_API int mivos_memory_read_dense_sets(const float* bank_k, const
                 out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
   int rc = memread_sets_args(a, sets, "memory_read_dense_sets");
   if (rc == MIVOS_OK) rc = memread_check_args(a, "memory_read_dense_sets");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_dense_run(a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" MIVOS_API int mivos_memory_read_dense_groups(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                        int k_objects, int64_t slots, const float* qk, int hw,
+                                                        int groups, const int32_t* first, void* out, int out_cstride,
+                                                        int out_coff, int out_halo_h, int out_halo_w, void* workspace,
+                                                        int64_t workspace_bytes, const int32_t* dyn_slots, int out_f16,
+                                                        mivos_stream_t stream_) {
+  MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, 0,
+                out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  int rc = memread_check_args(a, "memory_read_dense_groups");
+  if (rc == MIVOS_OK) rc = memread_groups_args(a, groups, first, "memory_read_dense_groups");
   if (rc != MIVOS_OK) return rc;
   return memory_read_dense_run(a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }

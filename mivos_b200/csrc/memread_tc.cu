@@ -36,6 +36,7 @@
 #include "sm90.cuh"
 
 #include <atomic>
+#include <type_traits>
 
 namespace mivos {
 extern std::atomic<int64_t> g_launches;
@@ -69,13 +70,19 @@ struct TcParams {
   int* tau_g;           // [K*hw] order-preserving int encoding of the best threshold any CTA has found
   int* err;
 };
+// The grouped form's block: the group table follows (a separate type, so the other instantiations keep theirs).
+struct TcGroupParams : TcParams {
+  const int* first;  // [groups + 1] device table (groups.cuh)
+  int groups, k_objects;
+};
 
 // ---- prep: scaled queries, their norms, and the max key norm per object --------------------
 __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_rows, int q_div, float* __restrict__ qs,
                                     float* __restrict__ qnorm, const float* __restrict__ bank_k,
                                     int64_t slots_cap, int64_t slots, int k_objects,
                                     unsigned int* __restrict__ kmax2_bits, int qblocks,
-                                    const int* __restrict__ dyn_slots, int dyn_set_stride, int* __restrict__ tau_g) {
+                                    const int* __restrict__ dyn_slots, int dyn_set_stride, int* __restrict__ tau_g,
+                                    const int* __restrict__ first, int groups) {
   mivos::pdl_prologue();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (static_cast<int>(blockIdx.x) < qblocks) {
@@ -92,8 +99,14 @@ __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_
       if (lane == 0) qnorm[r] = sqrtf(n2) * 1.0001f;  // round the bound up
       // shared thresholds of the objects that read this query set start at the lowest value
       const int set = r / hw, q = r - set * hw;
-      const int o0 = q_div > 0 ? set * q_div : 0;
-      int o1 = q_div > 0 ? o0 + q_div : k_objects;
+      int o0, o1;
+      if (first) {  // object groups: the set's group, nothing for a group outside [0, k_objects]
+        if (!group_range(first, k_objects, set, &o0, &o1)) o1 = 0;
+        o1 += o0;
+      } else {
+        o0 = q_div > 0 ? set * q_div : 0;
+        o1 = q_div > 0 ? o0 + q_div : k_objects;
+      }
       if (o1 > k_objects) o1 = k_objects;
       for (int o = o0 + lane; o < o1; o += 32) tau_g[static_cast<int64_t>(o) * hw + q] = float_ordered(-3.0e38f);
     }
@@ -104,7 +117,8 @@ __global__ void memread_prep_kernel(const float* __restrict__ qk, int hw, int q_
   const int b = blockIdx.x - qblocks;
   for (int obj = 0; obj < k_objects; ++obj) {
     // the bound covers the live keys of this object's set only
-    const int64_t live = live_slots(dyn_slots, slots, slots_cap, q_div > 0 ? obj / q_div : 0, dyn_set_stride);
+    const int g = first ? map_group(first, groups, k_objects, obj) : (q_div > 0 ? obj / q_div : 0);
+    const int64_t live = g < 0 ? 0 : live_slots(dyn_slots, slots, slots_cap, g, dyn_set_stride);
     float best = 0.f;
     for (int64_t s = static_cast<int64_t>(b) * 8 + warp; s < live; s += static_cast<int64_t>(nb) * 8) {
       const float4 v = reinterpret_cast<const float4*>(bank_k + (static_cast<int64_t>(obj) * slots_cap + s) * 128)[lane];
@@ -216,11 +230,12 @@ constexpr int STG_BYTES = 64 * STG_STRIDE * 4;
 // launch is refused.  The 128-float accumulator fragment, the NB bucket maxima and a 32-score chunk do not all fit
 // there: ptxas spills 0.3-1.3 KB per thread (NB = 32 / 64), served from L1, inside the candidate loop.
 // SETS: per-set counts (query set s reads its count from dyn_slots[s]).  A template flag, not a TcParams field, so
-// the scalar instantiations keep their parameter block and register allocation.
-template <int NB, bool SETS>
+// the scalar instantiations keep their parameter block and register allocation.  GROUPS (with SETS): object o reads
+// the query set and count of its group in the table of TcGroupParams.
+template <int NB, bool SETS, bool GROUPS = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                  const TcParams p) {
+                  const std::conditional_t<GROUPS, TcGroupParams, TcParams> p) {
   mivos::pdl_prologue();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -238,9 +253,17 @@ memread_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const int q0 = blockIdx.x * TQ;
   const int split = blockIdx.y;
   const int obj = blockIdx.z;
-  const int qset = p.q_div > 0 ? obj / p.q_div : 0;
+  int qset;
+  int64_t slots;
+  if constexpr (GROUPS) {  // an object in no group reads set 0 over no slot
+    const int g = map_group(p.first, p.groups, p.k_objects, obj);
+    qset = g < 0 ? 0 : g;
+    slots = g < 0 ? 0 : live_slots(p.dyn_slots, p.slots, p.slots_cap, g, 1);
+  } else {
+    qset = p.q_div > 0 ? obj / p.q_div : 0;
+    slots = live_slots(p.dyn_slots, p.slots, p.slots_cap, SETS ? qset : 0, SETS ? 1 : 0);
+  }
   const int qrow0 = qset * p.hw;  // first row of this object's query set
-  const int64_t slots = live_slots(p.dyn_slots, p.slots, p.slots_cap, SETS ? qset : 0, SETS ? 1 : 0);
   const int total_tiles = static_cast<int>((slots + TS - 1) / TS);
   // with a device-side slot count the grid (splits) is fixed by the host for the bank capacity and
   // the tile ranges are derived here; splits beyond the live bank publish empty lists and leave
@@ -473,7 +496,7 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
   float* qs = reinterpret_cast<float*>(w + ws.off_qs);
   float* qnorm = reinterpret_cast<float*>(w + ws.off_qnorm);
   int* tau_g = reinterpret_cast<int*>(w + ws.off_tau);
-  const int q_sets = a.q_div > 0 ? ceil_div(a.k_objects, a.q_div) : 1;
+  const int q_sets = a.first ? a.groups : a.q_div > 0 ? ceil_div(a.k_objects, a.q_div) : 1;
   const int q_rows = q_sets * a.hw;
 
   // overflow flags (written here and by the first selection pass, read by the exact fallback and the second selection
@@ -483,7 +506,7 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
   const int qblocks = ceil_div(q_rows, 8);
   const int kblocks = 296;
   launch_pdl(memread_prep_kernel, qblocks + kblocks, 256, 0, stream, a.qk, a.hw, q_rows, a.q_div, qs, qnorm, a.bank_k,
-             a.slots_cap, a.slots, a.k_objects, kmax2, qblocks, a.dyn_slots, a.dyn_set_stride, tau_g);
+             a.slots_cap, a.slots, a.k_objects, kmax2, qblocks, a.dyn_slots, a.dyn_set_stride, tau_g, a.first, a.groups);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 
@@ -493,7 +516,7 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
   rc = encode_tmap_2d(&tmK, a.bank_k, static_cast<uint64_t>(a.k_objects) * a.slots_cap, 128, 128, KB, TS);
   if (rc != MIVOS_OK) return rc;
 
-  TcParams p;
+  TcGroupParams p;
   p.slots_cap = a.slots_cap;
   p.slots = a.slots;
   p.dyn_slots = a.dyn_slots;
@@ -510,6 +533,10 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
   p.overflow = flags;
   p.tau_g = tau_g;
   p.err = device_error_flag();
+  p.first = a.first;
+  p.groups = a.groups;
+  p.k_objects = a.k_objects;
+  const TcParams& ps = p;
 
   static bool configured = false;
   if (!configured) {
@@ -517,14 +544,20 @@ int memread_tc_run(const MemreadArgs& a, int top_k, int32_t* topk_idx, float* to
     MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
     MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
     MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<32, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       TC_SMEM));
+    MIVOS_CUDA_OK(cudaFuncSetAttribute(memread_tc_kernel<64, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       TC_SMEM));
     configured = true;
   }
   dim3 grid(tc.qtiles, tc.splits, a.k_objects);
   const bool sets = a.dyn_set_stride != 0;
-  if (top_k <= 32 && !sets) launch_pdl(memread_tc_kernel<32, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-  else if (!sets) launch_pdl(memread_tc_kernel<64, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-  else if (top_k <= 32) launch_pdl(memread_tc_kernel<32, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
-  else launch_pdl(memread_tc_kernel<64, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  if (a.first && top_k <= 32) launch_pdl(memread_tc_kernel<32, true, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  else if (a.first) launch_pdl(memread_tc_kernel<64, true, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, p);
+  else if (top_k <= 32 && !sets) launch_pdl(memread_tc_kernel<32, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, ps);
+  else if (!sets) launch_pdl(memread_tc_kernel<64, false>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, ps);
+  else if (top_k <= 32) launch_pdl(memread_tc_kernel<32, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, ps);
+  else launch_pdl(memread_tc_kernel<64, true>, grid, TC_THREADS, TC_SMEM, stream, tmQ, tmK, ps);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   MIVOS_CUDA_OK(cudaGetLastError());
 

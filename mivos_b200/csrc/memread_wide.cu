@@ -91,7 +91,7 @@ memread_wide_sweep_kernel(const MemreadArgs a, const int splits, const WideState
 
   if (LEVEL < 2)
     for (int i = tid; i < WQ * kBins; i += W_THREADS) (&sm.hist[0][0])[i] = 0u;
-  const int qset = a.q_div > 0 ? obj / a.q_div : 0;
+  const int qset = query_set(a, obj);
   const float* qk = a.qk + (static_cast<int64_t>(qset) * hw + q0) * 128;
   for (int i = tid; i < WQ * 128; i += W_THREADS) {
     const int q = i >> 7, c = i & 127;
@@ -354,8 +354,9 @@ memread_wide_select_kernel(const MemreadArgs a, const int top_k, const WideState
   const int64_t lq = blockIdx.x;
   const int hw = a.hw;
   const int obj = static_cast<int>(lq / hw), q = static_cast<int>(lq - static_cast<int64_t>(obj) * hw);
-  const int qset = a.q_div > 0 ? obj / a.q_div : 0;
-  const int64_t live = live_slots(a, obj);
+  const int grp = object_group(a, obj);  // -1: in no group, reads set 0 over no slot
+  const int qset = grp < 0 ? 0 : grp;
+  const int64_t live = grp < 0 ? 0 : live_slots(a.dyn_slots, a.slots, a.slots_cap, grp, a.dyn_set_stride);
 
   int n;
   if (state[lq].mode != 2) {
@@ -550,6 +551,21 @@ extern "C" MIVOS_API int mivos_memory_read_wide_sets(const float* bank_k, const 
                 out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
   int rc = memread_sets_args(a, sets, "memory_read_wide_sets");
   if (rc == MIVOS_OK) rc = memread_check_args(a, "memory_read_wide_sets");
+  if (rc != MIVOS_OK) return rc;
+  return memory_read_wide_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes,
+                              reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" MIVOS_API int mivos_memory_read_wide_groups(const float* bank_k, const float* bank_v, int64_t slots_cap,
+                                                       int k_objects, int64_t slots, const float* qk, int hw, int groups,
+                                                       const int32_t* first, int top_k, void* out, int out_cstride,
+                                                       int out_coff, int out_halo_h, int out_halo_w, int32_t* topk_idx,
+                                                       float* topk_val, void* workspace, int64_t workspace_bytes,
+                                                       const int32_t* dyn_slots, int out_f16, mivos_stream_t stream_) {
+  MemreadArgs a{bank_k, bank_v, slots_cap, k_objects, slots, dyn_slots, qk, hw, 0,
+                out, out_cstride, out_coff, out_halo_h, out_halo_w, out_f16, 0};
+  int rc = memread_check_args(a, "memory_read_wide_groups");
+  if (rc == MIVOS_OK) rc = memread_groups_args(a, groups, first, "memory_read_wide_groups");
   if (rc != MIVOS_OK) return rc;
   return memory_read_wide_run(a, top_k, topk_idx, topk_val, workspace, workspace_bytes,
                               reinterpret_cast<cudaStream_t>(stream_));

@@ -365,16 +365,22 @@ class PropagationEngine(_ResNetTrunk):
         self.encode_query_batch(frame.reshape(1, 3, H, W), qs)
         return qs
 
-    def encode_memory(self, frames: torch.Tensor, masks: torch.Tensor, objs: Optional[Tuple[int, int]] = None) -> torch.Tensor:
+    def encode_memory(self, frames: torch.Tensor, masks: torch.Tensor, objs: Optional[Tuple[int, int]] = None,
+                      first: Optional[torch.Tensor] = None, maps: int = 0) -> torch.Tensor:
         """memorize (prop_net.py:144-162) of one clip (frame [1,3,H,W], masks [K,1,H,W]) or of C clips (frames
         [C,3,H,W], masks [C,K,1,H,W], any clip stride): returns the HALO [C*K,H/16,W/16,640] key|value map, clip-major
         (a workspace buffer: consume before the next call).  The "others" channel sums over the objects of the SAME
         clip: the stem gather takes the C (frame, K masks) groups in one launch.  `objs` (k0, n), one clip only:
-        objects [k0, k0 + n) alone ([n,...] map), their "others" channels still summed over all K masks."""
+        objects [k0, k0 + n) alone ([n,...] map), their "others" channels still summed over all K masks.
+        `first` (object groups: C clips of different object counts): masks are the packed planes [maps + C,1,H,W]
+        (each clip's background plane, then its objects), clip g owns maps [first[g], first[g+1])."""
         H, W = masks.shape[-2:]
-        N = masks.shape[:-3].numel()  # K, or C*K
+        N = maps if first is not None else masks.shape[:-3].numel()  # K, or C*K
         pcs = self.pc["mask_rgb_encoder.conv1"]
-        if objs is None or objs == (0, N):
+        if first is not None:
+            stem = self.ws.mat("stem_m", N * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
+            ops.stem_gather_groups(frames, masks, N, first, stem)
+        elif objs is None or objs == (0, N):
             stem = self.ws.mat("stem_m", N * (H // 2 + 2) * (W // 2 + 2), pcs.cin_pad)
             ops.stem_gather(frames.reshape(-1, 3, H, W), masks, stem, s2d=True)
         else:
@@ -388,11 +394,18 @@ class PropagationEngine(_ResNetTrunk):
         return kv
 
     def memorize_into(self, frames: torch.Tensor, masks: torch.Tensor, bank_k, bank_v, t: int, dyn_t=None,
-                      dyn_sets: bool = False) -> None:
+                      dyn_sets: bool = False, first: Optional[torch.Tensor] = None) -> None:
         """encode_memory + bank_write into bank frame `t` (or the device scalar dyn_t, t its largest value) for every
         object: C clips of K <= CHUNK_OBJECTS objects in one batch, one clip of more objects in object_chunks.
-        dyn_sets (C clips, masks [C,K,1,H,W]): dyn_t holds one frame per clip, clip c writes frame dyn_t[c]."""
+        dyn_sets (C clips, masks [C,K,1,H,W]): dyn_t holds one frame per clip, clip c writes frame dyn_t[c].
+        `first` (object groups): masks the packed planes [N + C,1,H,W] of C clips of different object counts, bank
+        rows [0, N); clip g writes frame dyn_t[g]."""
         H, W = masks.shape[-2:]
+        if first is not None:
+            N = bank_k.shape[0]
+            kv = self.encode_memory(frames, masks, first=first, maps=N)
+            ops.bank_write_groups(kv, N, H // 16, W // 16, 0, 128, bank_k, bank_v, t, dyn_t, first)
+            return
         N = masks.shape[:-3].numel()
         if dyn_sets:
             kv = self.encode_memory(frames, masks)
@@ -423,12 +436,29 @@ class PropagationEngine(_ResNetTrunk):
         return 1 if self.top_k is None else self.top_k
 
     def _memory_read(self, bank_k, bank_v, slots: int, qk, n: int, cat, h16: int, w16: int, dyn_slots, q_div: int,
-                     dyn_sets: bool = False):
+                     dyn_sets: bool = False, first: Optional[torch.Tensor] = None):
         """The memory read of n objects into channels [0, 512) of `cat`: the top-k read (prop_net.py:47-73) for
         top_k <= 64, the wide top-k read above that, or the dense read of the reference's top_k=None
         (prop_net.py:99-102).  The only place that tells them apart.  dyn_sets: qk [sets,hw,128] and one live slot
-        count per set in dyn_slots (the per-set forms)."""
+        count per set in dyn_slots (the per-set forms).  `first`: qk [groups,hw,128], one count per group, and the
+        group table (the grouped forms)."""
         hw = h16 * w16
+        if first is not None:
+            nf = self.ws.full(n)
+            if self.top_k is None:
+                wsp = self.ws.raw("memread_dense", ops.memory_read_dense_workspace_bytes(nf, bank_k.shape[1], hw))
+                ops.memory_read_dense_groups(bank_k, bank_v, slots, qk, cat, dyn_slots, first, halo_hw=(h16, w16),
+                                             workspace=wsp)
+            elif self.top_k > ops.TOPK_READ_MAX_K:
+                wsp = self.ws.raw("memread_wide",
+                                  ops.memory_read_wide_workspace_bytes(nf, bank_k.shape[1], hw, self.top_k))
+                ops.memory_read_wide_groups(bank_k, bank_v, slots, qk, self.top_k, cat, dyn_slots, first,
+                                            halo_hw=(h16, w16), workspace=wsp)
+            else:
+                wsp = self.ws.raw("memread", ops.memory_read_workspace_bytes(nf, slots, hw, self.top_k))
+                ops.memory_read_groups(bank_k, bank_v, slots, qk, self.top_k, cat, dyn_slots, first, halo_hw=(h16, w16),
+                                       workspace=wsp, algo=self.memread_algo)
+            return
         if dyn_sets:
             nf = self.ws.full(n)  # a prefix batch reads through the full batch's workspace
             if self.top_k is None:
@@ -461,7 +491,7 @@ class PropagationEngine(_ResNetTrunk):
                             algo=self.memread_algo, dyn_slots=dyn_slots, q_div=q_div)
 
     def segment(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int = 1, *, prob_out=None, want_raw=False,
-                want_prob=True, dyn_slots=None, dyn_sets: bool = False):
+                want_prob=True, dyn_slots=None, dyn_sets: bool = False, first: Optional[torch.Tensor] = None):
         """segment_with_query (prop_net.py:170-181) + aggregate_wbg(keep_bg=True) (inference_core.py:175) for C
         clips.  The C*K object maps (clip-major: map c*K + k is object k of clip c) go through every convolution as
         ONE batch — the 1/16- and 1/8-resolution layers of a single clip have 14-54 row tiles for 132 SMs — while the
@@ -471,8 +501,14 @@ class PropagationEngine(_ResNetTrunk):
         bank_k/bank_v [C*K, cap, 128/512]; `q` the QueryState of one clip's frame, or for C > 1 the batched state of
         the C current frames (new_query_states(H, W, C)).  Returns (raw sigmoid [C*K,1,H,W] | None, prob
         [(K+1),1,H,W] | None), prob [C,K+1,1,H,W] for C > 1.  dyn_sets: `q` is a batched state of C >= 1 clips and
-        dyn_slots holds one live slot count per clip (the per-set read)."""
+        dyn_slots holds one live slot count per clip (the per-set read).  `first` (object groups, C clips of
+        different object counts): K is the number of object maps, clip g owns maps [first[g], first[g+1]) and the
+        device table `first` [C+1] is read at run time; prob_out is the packed [K + C,1,H,W] (each clip's background
+        plane, then its objects).  Returns (None, prob_out)."""
         H, W = q.h, q.w
+        if first is not None:
+            lg = self._decode(bank_k, bank_v, slots, q, K, C, dyn_slots, None, first=first)
+            return ops.upsample4x_sigmoid_aggregate_groups(lg, K, H // 4, W // 4, first, prob_out=prob_out)
         chunks = object_chunks(K) if C == 1 else [(0, K)]
         if dyn_sets:
             lg = self._decode(bank_k, bank_v, slots, q, K, C, dyn_slots, None, dyn_sets=True)
@@ -485,17 +521,21 @@ class PropagationEngine(_ResNetTrunk):
         return ops.upsample4x_sigmoid_aggregate_any(lg, K, H // 4, W // 4, want_raw=want_raw, want_prob=want_prob,
                                                     prob_out=prob_out, groups=C)
 
-    def _decode(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int, dyn_slots, lg, dyn_sets: bool = False):
+    def _decode(self, bank_k, bank_v, slots: int, q: QueryState, K: int, C: int, dyn_slots, lg, dyn_sets: bool = False,
+                first: Optional[torch.Tensor] = None):
         """Memory read and decoder of C*K object maps as one batch; returns their decoder.pred logits in `lg` (a
-        workspace map when None)."""
+        workspace map when None).  `first` (object groups): K is the number of maps, clip g owns [first[g], first[g+1])."""
         ws, pc = self.ws, self.pc
         H, W = q.h, q.w
         h16, w16 = H // 16, W // 16
-        N = C * K
+        N = K if first is not None else C * K
         cat = ws.halo("cat", N, h16, w16, 1024)
         # ONE read for the C clips: object c*K + k reads query set c (q_div = K objects per set; one clip: q_div 0)
-        self._memory_read(bank_k, bank_v, slots, q.qk, N, cat, h16, w16, dyn_slots, K if C > 1 else 0, dyn_sets)
-        ops.halo_copy(q.kv, cat, N, h16, w16, 512, src_coff=128, dst_coff=512)  # cat([readout, v16]) :178-179
+        self._memory_read(bank_k, bank_v, slots, q.qk, N, cat, h16, w16, dyn_slots, K if C > 1 else 0, dyn_sets, first)
+        if first is not None:
+            ops.halo_copy_groups(q.kv, cat, N, h16, w16, 512, first, src_coff=128, dst_coff=512)
+        else:
+            ops.halo_copy(q.kv, cat, N, h16, w16, 512, src_coff=128, dst_coff=512)  # cat([readout, v16]) :178-179
         catr = ws.halo("catr", N, h16, w16, 1024)
         ops.halo_copy(cat, catr, N, h16, w16, 1024, relu=True)
         x16 = ws.halo("dec16", N, h16, w16, 512)
@@ -503,20 +543,24 @@ class PropagationEngine(_ResNetTrunk):
         # up_16_8 / up_8_4 (modules.py:100-104): the skip paths were produced by the query pass (q.s8 / q.s4, one map
         # per clip); the reference broadcasts them over the objects in the add
         x8 = ws.halo("dec8", N, H // 8, W // 8, 256)
-        self._upblock_tail("decoder.up_16_8", q.s8, x16, N, H // 8, W // 8, 512, 256, x8, final_relu=False)
+        self._upblock_tail("decoder.up_16_8", q.s8, x16, N, H // 8, W // 8, 512, 256, x8, final_relu=False, first=first)
         x4 = ws.halo("dec4", N, H // 4, W // 4, 256)
-        self._upblock_tail("decoder.up_8_4", q.s4, x8, N, H // 4, W // 4, 256, 256, x4, final_relu=True)
+        self._upblock_tail("decoder.up_8_4", q.s4, x8, N, H // 4, W // 4, 256, 256, x4, final_relu=True, first=first)
         if lg is None:
             lg = ws.halo("logit", N, H // 4, W // 4, 32, torch.float32)
         _cg(ws, x4, pc["decoder.pred"], N, H // 4, W // 4, lg)
         return lg
 
-    def _upblock_tail(self, p, s2_skip, up, K, h, w, up_c, out_c, out, final_relu):
-        """x = skip (one map per frame, broadcast over that frame's objects) + bilinear_x2(up); out_conv ResBlock."""
+    def _upblock_tail(self, p, s2_skip, up, K, h, w, up_c, out_c, out, final_relu, first=None):
+        """x = skip (one map per frame, broadcast over that frame's objects) + bilinear_x2(up); out_conv ResBlock.
+        `first`: the skip map of frame g is broadcast over the maps of object group g."""
         ws = self.ws
         s2 = ws.halo("ub_s2", K, h, w, up_c)
         s2r = ws.halo("ub_s2r", K, h, w, up_c)
-        ops.upsample2x_add(s2, up, K, h, w, x_relu=s2r, skip=s2_skip)
+        if first is not None:
+            ops.upsample2x_add_groups(s2, up, K, h, w, s2_skip, first, x_relu=s2r)
+        else:
+            ops.upsample2x_add(s2, up, K, h, w, x_relu=s2r, skip=s2_skip)
         return self._resblock(f"{p}.out_conv", s2, s2r, K, h, w, up_c, out_c, out, out_relu_only=final_relu)
 
 

@@ -24,7 +24,8 @@ class FrameStep:
     cached on the network's engine and shared by successive sessions — the reference also shares the networks between
     sessions (eval_interactive_davis.py:83)."""
 
-    def __init__(self, net, C: int, K: int, nh: int, nw: int, cap_frames: int, lane: int = 0, ragged: bool = False):
+    def __init__(self, net, C: int, K: int, nh: int, nw: int, cap_frames: int, lane: int = 0, ragged: bool = False,
+                 maps: Optional[int] = None):
         eng = net.engine()
         dev = eng.device
         # the step is cached on the network's engine: a strong reference back would be a cycle that keeps a dropped
@@ -33,15 +34,21 @@ class FrameStep:
         self.C, self.K, self.nh, self.nw, self.lane = C, K, nh, nw, lane
         self.hw = (nh // 16) * (nw // 16)
         self.cap_frames = cap_frames
+        # mixed object counts (ragged, `maps` = the clips' total object count): bank rows, result planes and
+        # destination pointers are sized for the maps, not for C*K; the planes are PACKED [maps + C,1,nh,nw] (each
+        # clip's background plane, then its objects) and a device table `first` [C+1] says which clip owns which
+        self.maps = maps
+        N, P = (C * K, C * (K + 1)) if maps is None else (maps, maps + C)
         self.frames = torch.zeros((C, 3, nh, nw), dtype=torch.float32, device=dev)
-        self.prob = torch.zeros((C, K + 1, 1, nh, nw), dtype=torch.float32, device=dev)
+        self.prob = torch.zeros(((C, K + 1) if maps is None else (P,)) + (1, nh, nw), dtype=torch.float32, device=dev)
         self.dyn = torch.zeros(4, dtype=torch.int32, device=dev)
         states, self.batch = eng.new_query_states(nh, nw, C)
         # one clip keeps the single-clip operands: [hw,128] query keys (read without query sets), [K+1,1,H,W] planes
-        self.q, self.out = (states[0], self.prob[0]) if C == 1 else (self.batch, self.prob)
-        self.masks = self.out.narrow(-4, 1, K)  # the object planes the memorize reads
-        self.bank_k = torch.empty((C * K, cap_frames * self.hw, 128), dtype=torch.float32, device=dev)
-        self.bank_v = torch.empty((C * K, cap_frames * self.hw, 512), dtype=torch.float32, device=dev)
+        if maps is None:
+            self.q, self.out = (states[0], self.prob[0]) if C == 1 else (self.batch, self.prob)
+            self.masks = self.out.narrow(-4, 1, K)  # the object planes the memorize reads
+        self.bank_k = torch.empty((N, cap_frames * self.hw, 128), dtype=torch.float32, device=dev)
+        self.bank_v = torch.empty((N, cap_frames * self.hw, 512), dtype=torch.float32, device=dev)
         self.graphs = {}
         self.kernels = {}  # kernels per replay, for mivos_launch_count accounting
         # False: eager launches even when the caller asks for graph replay (bench.py's per-launch brackets)
@@ -56,28 +63,34 @@ class FrameStep:
         self.g_fixed = i64([t.data_ptr() for t in staged])
         self.g_bytes_host = [t.numel() * t.element_size() for t in staged]
         self.g_bytes = i64(self.g_bytes_host)
-        self.s_fixed = i64([self.prob[c, j].data_ptr() for c in range(C) for j in range(K + 1)])
+        planes = self.prob.view(P, 1, nh, nw)
+        self.s_fixed = i64([planes[j].data_ptr() for j in range(P)])
         self.plane_bytes = nh * nw * 4
-        self.s_bytes = i64([self.plane_bytes] * (C * (K + 1)))
+        self.s_bytes = i64([self.plane_bytes] * P)
         # ragged (clips with their own pass plans, LockstepSession): C more words of the table hold one live slot
         # count and one memorize frame per clip, as int32 `counts` [2C] = (slots of clips 0..C-1, frames of clips
         # 0..C-1), written with the pointers; a tick of the first n of the C clips runs over their leading rows
-        self.ragged = ragged
-        self.dynp = torch.zeros(C * (6 + K) + (C if ragged else 0), dtype=torch.int64, device=dev)
-        self.counts = self.dynp[C * (6 + K):].view(torch.int32) if ragged else None
+        # (mixed: (C + 2) // 2 more words hold the int32 group table `first` [C+1] of the tick's clip order)
+        self.ragged = ragged or maps is not None
+        words = 5 * C + P
+        self.dynp = torch.zeros(words + (C if self.ragged else 0) + ((C + 2) // 2 if maps is not None else 0),
+                                dtype=torch.int64, device=dev)
+        self.counts = self.dynp[words:words + C].view(torch.int32) if self.ragged else None
+        self.first = self.dynp[words + C:].view(torch.int32)[:C + 1] if maps is not None else None
 
     @staticmethod
-    def get(net, C: int, K: int, nh: int, nw: int, need_frames: int, lane: int = 0, ragged: bool = False) -> "FrameStep":
+    def get(net, C: int, K: int, nh: int, nw: int, need_frames: int, lane: int = 0, ragged: bool = False,
+            maps: Optional[int] = None) -> "FrameStep":
         """The cached step for these shapes.  Single clips are kept in the engine's `_frame_steps` (4 entries),
         lock-step groups, whose C*K banks are C times larger, in `_lock_steps` (2 entries); least recently used
         first out."""
         name, bound = ("_frame_steps", 4) if C == 1 else ("_lock_steps", 2)
         cache = net.engine().__dict__.setdefault(name, {})
         cap = (need_frames + 15) // 16 * 16
-        key = (C, K, nh, nw, cap, lane) + (("ragged",) if ragged else ())
+        key = (C, K, nh, nw, cap, lane) + (("ragged",) if ragged else ()) + (("maps", maps) if maps is not None else ())
         step = cache.pop(key, None)
         if step is None:
-            step = FrameStep(net, C, K, nh, nw, cap, lane, ragged)
+            step = FrameStep(net, C, K, nh, nw, cap, lane, ragged, maps)
             while len(cache) >= bound:  # dict order = use order
                 cache.pop(next(iter(cache)))
         cache[key] = step  # (re)insert as most recently used
@@ -113,8 +126,26 @@ class FrameStep:
                                       dyn_sets=True)
             ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, n * (K + 1), False, self.plane_bytes)
 
+    def _body_mixed(self, n: int, n_mem: int, mn: int, mm: int):
+        """A tick of the first n clips of a mixed step, the first n_mem memorizing: _body_ragged over object groups.
+        The clips' mn (mm) object maps are the leading bank rows and planes; the reads, the decoder's per-clip
+        operators, the aggregation, the memorize stem and the bank write take the group table `first`."""
+        eng, C, N = self.net.engine(), self.C, self.maps
+        with eng.lane(self.lane):
+            ws = eng.ws
+            ops.copy_segments(self.g_fixed, self.dynp, self.g_bytes, 5 * n, True, max(self.g_bytes_host))
+            with ws.prefix_of(mn, N):
+                eng.segment(self.bank_k[:mn], self.bank_v[:mn], self.cap_frames * self.hw, self.batch.first(n), mn, n,
+                            prob_out=self.prob[:mn + n], dyn_slots=self.counts[:n], first=self.first[:n + 1])
+            if n_mem:
+                with ws.prefix_of(mm, N):
+                    eng.memorize_into(self.frames[:n_mem], self.prob[:mm + n_mem], self.bank_k[:mm], self.bank_v[:mm],
+                                      self.cap_frames - 1, dyn_t=self.counts[C:C + n_mem], first=self.first[:n_mem + 1])
+            ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, mn + n, False, self.plane_bytes)
+
     def run_ragged(self, frames: Sequence[Optional[torch.Tensor]], cached, visible: Sequence[int],
-                   m_front: Sequence[int], n_mem: int, prob_dsts, ti: Sequence[int], graph: bool = True) -> torch.Tensor:
+                   m_front: Sequence[int], n_mem: int, prob_dsts, ti: Sequence[int], graph: bool = True,
+                   ks: Optional[Sequence[int]] = None) -> torch.Tensor:
         """One tick of the first n = len(cached) clips of a ragged step, each at its own frame: clip c reads
         visible[c] bank frames and (c < n_mem) memorizes into frame m_front[c]; frames[c] / cached[c] / ti[c] as in
         run, prob_dsts[c] clip c's destination volume or None (fused frame: the planes stay in self.prob[c]).  The
@@ -122,6 +153,12 @@ class FrameStep:
         assert self.ragged
         n, C, K = len(cached), self.C, self.K
         assert 1 <= n <= C and 0 <= n_mem <= n
+        mixed = self.maps is not None
+        if mixed:  # object counts of the clips in this tick's order, then of the rest of the C clips
+            assert ks is not None and len(ks) == C and sum(ks) == self.maps
+            first = [0]
+            for k in ks:
+                first.append(first[-1] + k)
         srcs, dsts, slots, mem_t = [], [], [], []
         for c in range(C):
             if c < n:
@@ -133,32 +170,38 @@ class FrameStep:
                 srcs += [frames[c].data_ptr() if c < n_mem else 0, q.kv.data_ptr(), q.qk.data_ptr(), q.s8.data_ptr(),
                          q.s4.data_ptr()]
                 d = prob_dsts[c]
-                dsts += [d[j, ti[c]].data_ptr() for j in range(K + 1)] if d is not None else [0] * (K + 1)
+                kc = ks[c] if mixed else K
+                dsts += [d[j, ti[c]].data_ptr() for j in range(kc + 1)] if d is not None else [0] * (kc + 1)
                 slots.append(visible[c] * self.hw)
                 mem_t.append(m_front[c] if c < n_mem else 0)
             else:
                 srcs += [0] * 5
-                dsts += [0] * (K + 1)
+                dsts += [0] * ((ks[c] if mixed else K) + 1)
                 slots.append(0)
                 mem_t.append(0)
         i32 = slots + mem_t
-        packed = [(i32[2 * i] & 0xFFFFFFFF) | ((i32[2 * i + 1] & 0xFFFFFFFF) << 32) for i in range(C)]
+        if mixed:
+            i32 += first + [0] * ((C + 2) // 2 * 2 - (C + 1))
+        packed = [(i32[2 * i] & 0xFFFFFFFF) | ((i32[2 * i + 1] & 0xFFFFFFFF) << 32) for i in range(len(i32) // 2)]
         packed = [w - (1 << 64) if w >= 1 << 63 else w for w in packed]
         ops.store_words(self.dynp, srcs + dsts + packed)
+        # a mixed step's graphs are keyed by the map counts of the two prefixes too (the table itself is device data)
+        args = (n, n_mem, first[n], first[n_mem]) if mixed else (n, n_mem)
+        body = self._body_mixed if mixed else self._body_ragged
         if not (graph and self.use_graph):
-            self._body_ragged(n, n_mem)
+            body(*args)
             return self.prob
         lib = _lib.load()
-        key = (n, n_mem)
+        key = args
         g = self.graphs.get(key)
         if g is None:
             n0 = lib.mivos_launch_count()
-            self._body_ragged(n, n_mem)
+            body(*args)
             self.kernels[key] = lib.mivos_launch_count() - n0
             torch.cuda.current_stream().synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._body_ragged(n, n_mem)
+                body(*args)
             lib.mivos_add_launch_count(-self.kernels[key])
             self.graphs[key] = g
             # the eager run above was this tick: a replay would run it twice, and a prefix first appears mid-pass,

@@ -367,13 +367,14 @@ def memory_read_workspace_bytes(k: int, slots: int, hw: int, top_k: int) -> int:
     return int(n)
 
 
-def _memread_operands(who: str, bank_k, bank_v, qk, out, q_div: int, halo_hw, workspace, need_bytes):
+def _memread_operands(who: str, bank_k, bank_v, qk, out, q_div: int, halo_hw, workspace, need_bytes,
+                      check_sets: bool = True):
     """What memory_read, memory_read_dense and memory_read_wide share: operand and query-set checks, (k, cap, hw), a workspace of at
     least need_bytes(k, cap, hw) bytes, and the halo dims ((0, 0): pixel-major output)."""
     _req(bank_k), _req(bank_v), _req(qk), _req_act(out)
     k, cap = bank_k.shape[0], bank_k.shape[1]
     hw = qk.shape[-2]
-    if qk.dim() == 3 and (q_div < 1 or (k + q_div - 1) // q_div != qk.shape[0]):
+    if check_sets and qk.dim() == 3 and (q_div < 1 or (k + q_div - 1) // q_div != qk.shape[0]):
         raise _lib.MivosError(f"{who}: {qk.shape[0]} query sets for {k} objects need q_div = objects per set (got {q_div})")
     if qk.dim() == 2 and q_div != 0:
         raise _lib.MivosError(f"{who}: q_div needs a [sets,hw,128] query tensor")
@@ -523,6 +524,145 @@ def _set_counts(who: str, qk: torch.Tensor, counts: torch.Tensor) -> int:
     if qk.dim() != 3 or counts.numel() < qk.shape[0]:
         raise _lib.MivosError(f"{who}: per-set counts need a [sets,hw,128] query tensor and one count per set")
     return qk.shape[0]
+
+
+# ---- object groups (lock-step clips with different object counts): `first` is an int32 device table of groups + 1
+# entries, group g owning maps [first[g], first[g+1]) (include/mivos_b200.h, "Object-group forms")
+
+def _group_table(who: str, first: torch.Tensor) -> int:
+    _req(first, torch.int32)
+    if first.dim() != 1 or first.numel() < 2:
+        raise _lib.MivosError(f"{who}: the group table holds groups + 1 >= 2 int32 entries")
+    return first.numel() - 1
+
+
+def _group_counts(who: str, qk: torch.Tensor, first: torch.Tensor, counts: torch.Tensor) -> int:
+    groups = _group_table(who, first)
+    _req(counts, torch.int32)
+    if qk.dim() != 3 or qk.shape[0] != groups or counts.numel() < groups:
+        raise _lib.MivosError(f"{who}: {groups} groups need a [groups,hw,128] query tensor and one count per group")
+    return groups
+
+
+def memory_read_groups(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, top_k: int,
+                       out: torch.Tensor, counts: torch.Tensor, first: torch.Tensor, *, out_coff: int = 0,
+                       halo_hw=None, workspace: Optional[torch.Tensor] = None, algo: int = MEMREAD_AUTO,
+                       want_topk: bool = False):
+    """memory_read of object groups: object o of group g (first[g] <= o < first[g+1]) reads query set g of qk
+    [groups,hw,128] over the live slots 0 .. counts[g] - 1 of its bank.  `slots` (>= top_k) sizes the launch."""
+    groups = _group_counts("memory_read_groups", qk, first, counts)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_groups", bank_k, bank_v, qk, out, 0, halo_hw, workspace,
+        lambda k, cap, hw: memory_read_workspace_bytes(k, slots, hw, top_k), check_sets=False)
+    idx = val = None
+    if want_topk:
+        idx = torch.empty((k, hw, top_k), dtype=torch.int32, device=qk.device)
+        val = torch.empty((k, hw, top_k), dtype=torch.float32, device=qk.device)
+    check(_lib.lib().mivos_memory_read_groups(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, groups,
+                                              _ptr(first), top_k, _ptr(out), out.shape[-1], out_coff, hh, ww, _ptr(idx),
+                                              _ptr(val), _ptr(workspace), workspace.numel(), algo, _ptr(counts),
+                                              _f16(out), _stream()), "mivos_memory_read_groups")
+    return (out, idx, val) if want_topk else out
+
+
+def memory_read_dense_groups(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor,
+                             out: torch.Tensor, counts: torch.Tensor, first: torch.Tensor, *, out_coff: int = 0,
+                             halo_hw=None, workspace: Optional[torch.Tensor] = None):
+    """memory_read_dense of object groups, as memory_read_groups."""
+    groups = _group_counts("memory_read_dense_groups", qk, first, counts)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_dense_groups", bank_k, bank_v, qk, out, 0, halo_hw, workspace, memory_read_dense_workspace_bytes,
+        check_sets=False)
+    check(_lib.lib().mivos_memory_read_dense_groups(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, groups,
+                                                    _ptr(first), _ptr(out), out.shape[-1], out_coff, hh, ww,
+                                                    _ptr(workspace), workspace.numel(), _ptr(counts), _f16(out),
+                                                    _stream()), "mivos_memory_read_dense_groups")
+    return out
+
+
+def memory_read_wide_groups(bank_k: torch.Tensor, bank_v: torch.Tensor, slots: int, qk: torch.Tensor, top_k: int,
+                            out: torch.Tensor, counts: torch.Tensor, first: torch.Tensor, *, out_coff: int = 0,
+                            halo_hw=None, workspace: Optional[torch.Tensor] = None, want_topk: bool = False):
+    """memory_read_wide of object groups, as memory_read_groups."""
+    groups = _group_counts("memory_read_wide_groups", qk, first, counts)
+    k, cap, hw, workspace, hh, ww = _memread_operands(
+        "memory_read_wide_groups", bank_k, bank_v, qk, out, 0, halo_hw, workspace,
+        lambda k, cap, hw: memory_read_wide_workspace_bytes(k, cap, hw, top_k), check_sets=False)
+    idx = val = None
+    if want_topk:
+        idx = torch.empty((k, hw, top_k), dtype=torch.int32, device=qk.device)
+        val = torch.empty((k, hw, top_k), dtype=torch.float32, device=qk.device)
+    check(_lib.lib().mivos_memory_read_wide_groups(_ptr(bank_k), _ptr(bank_v), cap, k, slots, _ptr(qk), hw, groups,
+                                                   _ptr(first), top_k, _ptr(out), out.shape[-1], out_coff, hh, ww,
+                                                   _ptr(idx), _ptr(val), _ptr(workspace), workspace.numel(),
+                                                   _ptr(counts), _f16(out), _stream()), "mivos_memory_read_wide_groups")
+    return (out, idx, val) if want_topk else out
+
+
+def bank_write_groups(halo: torch.Tensor, n: int, h: int, w: int, coff_k: int, coff_v: int, bank_k: torch.Tensor,
+                      bank_v: torch.Tensor, t_max: int, dyn_t: torch.Tensor, first: torch.Tensor) -> None:
+    """bank_write of n maps in object groups: group g writes its maps into bank frame dyn_t[g] (int32 device array,
+    read when the launch runs); `t_max` is the largest frame that may occur."""
+    groups = _group_table("bank_write_groups", first)
+    _req(halo), _req(bank_k), _req(bank_v), _req(dyn_t, torch.int32)
+    check(_lib.lib().mivos_bank_write_groups(_ptr(halo), n, groups, _ptr(first), h, w, halo.shape[-1], coff_k, coff_v,
+                                             _ptr(bank_k), _ptr(bank_v), bank_k.shape[1], t_max, _ptr(dyn_t),
+                                             _stream()), "mivos_bank_write_groups")
+
+
+def stem_gather_groups(frames: torch.Tensor, planes: torch.Tensor, n: int, first: torch.Tensor,
+                       out: torch.Tensor) -> torch.Tensor:
+    """The space-to-depth memorize stem of n object maps in groups: map i, object i - first[g] of group g, reads
+    frames[g] [G,3,H,W] and the packed planes [n + G,1,H,W] (group g: background first[g] + g, then its objects); its
+    "others" channel sums over group g's other objects."""
+    groups = _group_table("stem_gather_groups", first)
+    _req(frames), _req(planes), _req_act(out)
+    h, w = frames.shape[-2:]
+    check(_lib.lib().mivos_stem_gather_s2d_groups(_ptr(frames), _ptr(planes), n, groups, _ptr(first), h, w, _ptr(out),
+                                                  out.shape[-1], _f16(out), 3 * h * w, _stream()),
+          "mivos_stem_gather_s2d_groups")
+    return out
+
+
+def upsample2x_add_groups(x: torch.Tensor, up: torch.Tensor, n: int, h: int, w: int, skip: torch.Tensor,
+                          first: torch.Tensor, x_relu: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x = skip[g] + up2x(up) for the images of group g (upsample2x_add with skip maps broadcast over groups)."""
+    groups = _group_table("upsample2x_add_groups", first)
+    _req_act(x), _req_act(up), _req_act(skip)
+    assert x.shape[-1] == up.shape[-1] == skip.shape[-1]
+    check(_lib.lib().mivos_upsample2x_add_groups(_ptr(x), _ptr(up), n, h, w, x.shape[-1], _ptr(x_relu), _ptr(skip),
+                                                 groups, _ptr(first), _same_type(x, up, x_relu, skip), _stream()),
+          "mivos_upsample2x_add_groups")
+    return x
+
+
+def halo_copy_groups(src: torch.Tensor, dst: torch.Tensor, n: int, h: int, w: int, c: int, first: torch.Tensor, *,
+                     src_coff: int = 0, dst_coff: int = 0, relu: bool = False) -> torch.Tensor:
+    """halo_copy with source map g broadcast over the images of group g."""
+    groups = _group_table("halo_copy_groups", first)
+    _req_act(src), _req_act(dst)
+    check(_lib.lib().mivos_halo_copy_groups(_ptr(src), groups, _ptr(first), src.shape[-1], src_coff, _ptr(dst),
+                                            dst.shape[-1], dst_coff, n, h, w, c, int(relu), _f16(src), _f16(dst),
+                                            _stream()), "mivos_halo_copy_groups")
+    return dst
+
+
+def upsample4x_sigmoid_aggregate_groups(logits: torch.Tensor, n: int, h4: int, w4: int, first: torch.Tensor,
+                                        coff: int = 0, raw_out: Optional[torch.Tensor] = None,
+                                        prob_out: Optional[torch.Tensor] = None):
+    """upsample4x_sigmoid_aggregate of n maps in groups of at most 16: prob_out is the packed [n + G,1,H,W] (group g:
+    background plane first[g] + g, then its objects), raw_out [n,1,H,W]."""
+    groups = _group_table("upsample4x_sigmoid_aggregate_groups", first)
+    _req(logits)
+    if prob_out is None and raw_out is None:
+        prob_out = torch.empty((n + groups, 1, 4 * h4, 4 * w4), dtype=torch.float32, device=logits.device)
+    for t in (raw_out, prob_out):
+        if t is not None:
+            _req(t)
+    check(_lib.lib().mivos_upsample4x_sigmoid_aggregate_groups(_ptr(logits), n, groups, _ptr(first), h4, w4,
+                                                               logits.shape[-1], coff, _ptr(raw_out), _ptr(prob_out),
+                                                               _stream()), "mivos_upsample4x_sigmoid_aggregate_groups")
+    return raw_out, prob_out
 
 
 def upsample4x_sigmoid_aggregate(logits: torch.Tensor, k: int, h4: int, w4: int, coff: int = 0,
