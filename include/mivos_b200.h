@@ -77,6 +77,27 @@ MIVOS_API int mivos_store_words(int64_t* dst64, int n64, const int64_t* vals64, 
  * frame ti (InferenceCore.prob[:, ti], inference_core.py:194) without eager copies between graph replays.            */
 MIVOS_API int mivos_copy_segments(const int64_t* fixed, const int64_t* dyn, const int64_t* bytes, int n,
                         int dyn_is_src, int64_t max_bytes, mivos_stream_t stream);
+/* Result delivery to host volumes (InferenceCore(result_dev="cpu")): one launch delivers the result planes of every
+ * clip of a tick, reading each plane once from device memory.  `table` holds MIVOS_DELIVER_WORDS int64 words per
+ * clip, read on the device when the (captured) launch runs:
+ *   [0] address of the clip's probability volume at frame ti, prob[0, ti] of [(K+1), T, 1, nh, nw] fp32; 0 skips
+ *   [1] the volume's plane stride in elements (T * nh * nw)
+ *   [2] address of the padded label map at frame ti ([T, 1, nh, nw] u8)
+ *   [3] address of the unpadded label map at frame ti ([T, h, w] u8)
+ *   [4] low 32 bits: index of the clip's first plane in `planes`; high 32 bits: its plane count K+1 (1 to 256)
+ *   [5] pad_l | pad_t << 32      [6] h | w << 32      [7] unused
+ * Clip c copies planes[first + j] (j < K+1) to its volume's plane j at frame ti in 16-byte stores, and writes the
+ * frame's argmax over the K+1 planes (the first maximum wins, as mivos_argmax_unpad) padded and unpadded.  The
+ * destinations may be host-mapped addresses (mivos_host_register); volume, stride and padded labels must be 16-byte
+ * aligned.  A record whose plane count is out of range is skipped.  nh * nw must be a multiple of 16.           */
+#define MIVOS_DELIVER_WORDS 8
+MIVOS_API int mivos_deliver_planes(const float* planes, const int64_t* table, int clips, int nh, int nw,
+                         mivos_stream_t stream);
+/* Page-locks `bytes` of pageable host memory at `host` (cudaHostRegister, mapped and portable) and returns in
+ * *dev_out the address kernels use for it (cudaHostGetDevicePointer; not assumed equal to `host`).  Host code
+ * allocates the memory; the library allocates nothing.  mivos_host_unregister undoes it.                        */
+MIVOS_API int mivos_host_register(void* host, int64_t bytes, void** dev_out);
+MIVOS_API int mivos_host_unregister(void* host);
 
 /* Convolution as implicit GEMM on wgmma (TF32 in, FP32 accumulate) ----------------------------
  * Replaces nn.Conv2d (+ eval BatchNorm2d folded into weight/bias, + ReLU, + residual add) as

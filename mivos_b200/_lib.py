@@ -67,6 +67,9 @@ SIGNATURES = {
     "mivos_store_i32": (_i, [_p, _i, _i, _i, _i, _i, _p]),
     "mivos_store_words": (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _p]),
     "mivos_copy_segments": (_i, [_p, _p, _p, _i, _i, _l, _p]),
+    "mivos_deliver_planes": (_i, [_p, _p, _i, _i, _i, _p]),
+    "mivos_host_register": (_i, [_p, _l, C.POINTER(_p)]),
+    "mivos_host_unregister": (_i, [_p]),
     "mivos_conv_gemm": (_i, [C.POINTER(ConvArgs), _p]),
     "mivos_conv_tile_override": (_i, [_i, _i]),
     "mivos_conv_plan": (_i, [C.POINTER(ConvArgs), _i, C.POINTER(_i), C.POINTER(_i)]),

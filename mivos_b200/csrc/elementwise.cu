@@ -468,6 +468,65 @@ __global__ void copy_segments_kernel(const int64_t* __restrict__ fixed, const in
     dst[i] = src[i];
 }
 
+// Result delivery to (host-mapped) volumes: blockIdx.y = clip, its record of MIVOS_DELIVER_WORDS words in `table`
+// (header).  A thread owns 16 consecutive pixels of the padded plane: it reads each of the clip's K+1 planes once
+// (four 16-byte loads), stores them to the volume in 16-byte stores (a warp writes 2 KB contiguous per plane) and
+// keeps the running argmax, whose 16 labels go out as one 16-byte store.  The unpadded labels of the block's span
+// go through shared memory so that consecutive threads store consecutive bytes of a row.
+constexpr int kDeliverPix = 16;
+constexpr int kDeliverSpan = kThreads * kDeliverPix;
+__global__ void __launch_bounds__(kThreads) deliver_planes_kernel(const float* __restrict__ planes,
+                                                                  const int64_t* __restrict__ table, int nh, int nw) {
+  mivos::pdl_prologue();
+  __shared__ uint8_t lab[kDeliverSpan];
+  const int64_t* rec = table + static_cast<int64_t>(blockIdx.y) * MIVOS_DELIVER_WORDS;
+  float* prob = reinterpret_cast<float*>(rec[0]);
+  const int64_t stride = rec[1];
+  uint8_t* lp = reinterpret_cast<uint8_t*>(rec[2]);
+  uint8_t* lu = reinterpret_cast<uint8_t*>(rec[3]);
+  const int src0 = static_cast<int>(rec[4] & 0xFFFFFFFF), k1 = static_cast<int>(rec[4] >> 32);
+  const int pad_l = static_cast<int>(rec[5] & 0xFFFFFFFF), pad_t = static_cast<int>(rec[5] >> 32);
+  const int h = static_cast<int>(rec[6] & 0xFFFFFFFF), w = static_cast<int>(rec[6] >> 32);
+  if (prob == nullptr || k1 < 1 || k1 > MIVOS_MAX_OBJECTS + 1) return;  // uniform over the block
+  const int64_t plane = static_cast<int64_t>(nh) * nw;
+  const float* src = planes + static_cast<int64_t>(src0) * plane;
+  for (int64_t base = static_cast<int64_t>(blockIdx.x) * kDeliverSpan; base < plane;
+       base += static_cast<int64_t>(gridDim.x) * kDeliverSpan) {
+    const int64_t i = base + threadIdx.x * kDeliverPix;
+    if (i < plane) {
+      float best[kDeliverPix];
+      uint32_t arg[kDeliverPix / 4] = {0u, 0u, 0u, 0u};  // four labels per word, byte q%4 of word q/4
+      for (int j = 0; j < k1; ++j) {
+        const float4* s = reinterpret_cast<const float4*>(src + j * plane + i);
+        float4* d = reinterpret_cast<float4*>(prob + j * stride + i);
+#pragma unroll
+        for (int v = 0; v < kDeliverPix / 4; ++v) {
+          const float4 x = __ldg(s + v);
+          d[v] = x;
+          const float e[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const int q = v * 4 + u;
+            if (j == 0 || e[u] > best[q]) {
+              best[q] = e[u];
+              arg[v] = (arg[v] & ~(0xFFu << (8 * u))) | (static_cast<uint32_t>(j) << (8 * u));
+            }
+          }
+        }
+      }
+      *reinterpret_cast<uint4*>(lp + i) = make_uint4(arg[0], arg[1], arg[2], arg[3]);
+      *reinterpret_cast<uint4*>(lab + threadIdx.x * kDeliverPix) = make_uint4(arg[0], arg[1], arg[2], arg[3]);
+    }
+    __syncthreads();
+    for (int q = threadIdx.x; q < kDeliverSpan && base + q < plane; q += kThreads) {
+      const int64_t p = base + q;
+      const int y = static_cast<int>(p / nw) - pad_t, x = static_cast<int>(p % nw) - pad_l;
+      if (y >= 0 && y < h && x >= 0 && x < w) lu[static_cast<int64_t>(y) * w + x] = lab[q];
+    }
+    __syncthreads();
+  }
+}
+
 inline unsigned capped_grid(int64_t work) {
   // grid-stride kernels: a few waves of the SMs x 8 resident 256-thread CTAs is plenty
   const int64_t cap = num_sms() * 16ll;
@@ -722,6 +781,18 @@ extern "C" MIVOS_API int mivos_copy_segments(const int64_t* fixed, const int64_t
   MIVOS_REQUIRE(fixed && dyn && bytes && n >= 1 && n <= 65535 && max_bytes >= 16, "copy_segments: bad arguments");
   const dim3 grid(capped_grid(max_bytes / 16), n);
   launch_pdl(copy_segments_kernel, grid, kThreads, 0, ST(s), fixed, dyn, bytes, dyn_is_src);
+  MIVOS_LAUNCHED();
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_deliver_planes(const float* planes, const int64_t* table, int clips, int nh, int nw,
+                                              mivos_stream_t s) {
+  MIVOS_REQUIRE(planes && table && AL16(planes) && clips >= 1 && clips <= 65535 && nh >= 1 && nw >= 1 &&
+                    (static_cast<int64_t>(nh) * nw) % kDeliverPix == 0,
+                "deliver_planes: bad arguments (clips %d, %dx%d)", clips, nh, nw);
+  const int64_t spans = (static_cast<int64_t>(nh) * nw + kDeliverSpan - 1) / kDeliverSpan;
+  const dim3 grid(static_cast<unsigned>(spans < num_sms() * 4 ? spans : num_sms() * 4), clips);
+  launch_pdl(deliver_planes_kernel, grid, kThreads, 0, ST(s), planes, table, nh, nw);
   MIVOS_LAUNCHED();
   return MIVOS_OK;
 }

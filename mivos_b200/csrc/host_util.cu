@@ -144,6 +144,26 @@ bool pdl_enabled() {
 }
 }  // namespace mivos
 
+extern "C" MIVOS_API int mivos_host_register(void* host, int64_t bytes, void** dev_out) {
+  MIVOS_REQUIRE(host && bytes > 0 && dev_out, "host_register: bad arguments");
+  MIVOS_CUDA_OK(cudaHostRegister(host, static_cast<size_t>(bytes), cudaHostRegisterMapped | cudaHostRegisterPortable));
+  void* dev = nullptr;
+  const cudaError_t e = cudaHostGetDevicePointer(&dev, host, 0);
+  if (e != cudaSuccess) {
+    cudaHostUnregister(host);
+    set_last_error("host_register: cudaHostGetDevicePointer -> %s", cudaGetErrorString(e));
+    return MIVOS_ERR_CUDA;
+  }
+  *dev_out = dev;
+  return MIVOS_OK;
+}
+
+extern "C" MIVOS_API int mivos_host_unregister(void* host) {
+  MIVOS_REQUIRE(host, "host_unregister: null pointer");
+  MIVOS_CUDA_OK(cudaHostUnregister(host));
+  return MIVOS_OK;
+}
+
 extern "C" MIVOS_API int64_t mivos_launch_count(void) { return g_launches.load(); }
 
 // A replayed CUDA graph launches the kernels that were captured through this library without

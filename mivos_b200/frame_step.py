@@ -9,6 +9,7 @@ import torch
 
 from . import _lib, ops
 from ._lib import MivosError
+from .host_results import HostResults
 
 
 class FrameStep:
@@ -73,10 +74,13 @@ class FrameStep:
         # (mixed: (C + 2) // 2 more words hold the int32 group table `first` [C+1] of the tick's clip order)
         self.ragged = ragged or maps is not None
         words = 5 * C + P
-        self.dynp = torch.zeros(words + (C if self.ragged else 0) + ((C + 2) // 2 if maps is not None else 0),
-                                dtype=torch.int64, device=dev)
+        # host results (InferenceCore(result_dev="cpu")): one mivos_deliver_planes record per clip follows, written
+        # only in the ticks that have such a clip; a tick of device-result clips writes and launches what it always did
+        self.d_off = words + (C if self.ragged else 0) + ((C + 2) // 2 if maps is not None else 0)
+        self.dynp = torch.zeros(self.d_off + C * ops.DELIVER_WORDS, dtype=torch.int64, device=dev)
         self.counts = self.dynp[words:words + C].view(torch.int32) if self.ragged else None
         self.first = self.dynp[words + C:].view(torch.int32)[:C + 1] if maps is not None else None
+        self.records = self.dynp[self.d_off:]
 
     @staticmethod
     def get(net, C: int, K: int, nh: int, nw: int, need_frames: int, lane: int = 0, ragged: bool = False,
@@ -96,7 +100,7 @@ class FrameStep:
         cache[key] = step  # (re)insert as most recently used
         return step
 
-    def _body(self, memorize: bool):
+    def _body(self, memorize: bool, host: bool = False):
         eng, C, K = self.net.engine(), self.C, self.K
         with eng.lane(self.lane):
             ops.copy_segments(self.g_fixed, self.dynp, self.g_bytes, 5 * C, True, max(self.g_bytes_host))
@@ -107,8 +111,10 @@ class FrameStep:
                 eng.memorize_into(self.frames, self.masks, self.bank_k, self.bank_v, self.cap_frames - 1,
                                   dyn_t=self.dyn[1:2])
             ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, C * (K + 1), False, self.plane_bytes)
+            if host:
+                ops.deliver_planes(self.prob, self.records, C, self.nh, self.nw)
 
-    def _body_ragged(self, n: int, n_mem: int):
+    def _body_ragged(self, n: int, n_mem: int, host: bool = False):
         """A tick of the first n clips, the first n_mem of them memorizing: the same operators as _body over the
         leading n (n_mem) clips, the reads and the bank write in their per-set forms (counts per clip)."""
         eng, C, K = self.net.engine(), self.C, self.K
@@ -125,8 +131,10 @@ class FrameStep:
                                       self.bank_v[:n_mem * K], self.cap_frames - 1, dyn_t=self.counts[C:C + n_mem],
                                       dyn_sets=True)
             ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, n * (K + 1), False, self.plane_bytes)
+            if host:
+                ops.deliver_planes(self.prob, self.records, n, self.nh, self.nw)
 
-    def _body_mixed(self, n: int, n_mem: int, mn: int, mm: int):
+    def _body_mixed(self, n: int, n_mem: int, mn: int, mm: int, host: bool = False):
         """A tick of the first n clips of a mixed step, the first n_mem memorizing: _body_ragged over object groups.
         The clips' mn (mm) object maps are the leading bank rows and planes; the reads, the decoder's per-clip
         operators, the aggregation, the memorize stem and the bank write take the group table `first`."""
@@ -142,13 +150,16 @@ class FrameStep:
                     eng.memorize_into(self.frames[:n_mem], self.prob[:mm + n_mem], self.bank_k[:mm], self.bank_v[:mm],
                                       self.cap_frames - 1, dyn_t=self.counts[C:C + n_mem], first=self.first[:n_mem + 1])
             ops.copy_segments(self.s_fixed, self.dynp[5 * C:], self.s_bytes, mn + n, False, self.plane_bytes)
+            if host:
+                ops.deliver_planes(self.prob, self.records, n, self.nh, self.nw)
 
     def run_ragged(self, frames: Sequence[Optional[torch.Tensor]], cached, visible: Sequence[int],
                    m_front: Sequence[int], n_mem: int, prob_dsts, ti: Sequence[int], graph: bool = True,
                    ks: Optional[Sequence[int]] = None) -> torch.Tensor:
         """One tick of the first n = len(cached) clips of a ragged step, each at its own frame: clip c reads
         visible[c] bank frames and (c < n_mem) memorizes into frame m_front[c]; frames[c] / cached[c] / ti[c] as in
-        run, prob_dsts[c] clip c's destination volume or None (fused frame: the planes stay in self.prob[c]).  The
+        run, prob_dsts[c] clip c's destination volume, its HostResults, or None (fused frame: the planes stay in
+        self.prob[c]).  The
         pointers and the per-clip counters are written with one store; one captured graph per (n, n_mem)."""
         assert self.ragged
         n, C, K = len(cached), self.C, self.K
@@ -159,7 +170,7 @@ class FrameStep:
             first = [0]
             for k in ks:
                 first.append(first[-1] + k)
-        srcs, dsts, slots, mem_t = [], [], [], []
+        srcs, dsts, slots, mem_t, recs = [], [], [], [], []
         for c in range(C):
             if c < n:
                 assert visible[c] <= self.cap_frames and m_front[c] < self.cap_frames
@@ -171,6 +182,11 @@ class FrameStep:
                          q.s4.data_ptr()]
                 d = prob_dsts[c]
                 kc = ks[c] if mixed else K
+                if isinstance(d, HostResults):  # the clip's planes: packed (background, then its objects) or row c
+                    recs += d.record(ti[c], first[c] + c if mixed else c * (K + 1))
+                    d = None
+                else:
+                    recs += [0] * ops.DELIVER_WORDS
                 dsts += [d[j, ti[c]].data_ptr() for j in range(kc + 1)] if d is not None else [0] * (kc + 1)
                 slots.append(visible[c] * self.hw)
                 mem_t.append(m_front[c] if c < n_mem else 0)
@@ -184,24 +200,26 @@ class FrameStep:
             i32 += first + [0] * ((C + 2) // 2 * 2 - (C + 1))
         packed = [(i32[2 * i] & 0xFFFFFFFF) | ((i32[2 * i + 1] & 0xFFFFFFFF) << 32) for i in range(len(i32) // 2)]
         packed = [w - (1 << 64) if w >= 1 << 63 else w for w in packed]
-        ops.store_words(self.dynp, srcs + dsts + packed)
-        # a mixed step's graphs are keyed by the map counts of the two prefixes too (the table itself is device data)
+        host = any(recs)
+        ops.store_words(self.dynp, srcs + dsts + packed + (recs if host else []))
+        # a mixed step's graphs are keyed by the map counts of the two prefixes too (the table itself is device data),
+        # and every step's by the delivery kind
         args = (n, n_mem, first[n], first[n_mem]) if mixed else (n, n_mem)
         body = self._body_mixed if mixed else self._body_ragged
         if not (graph and self.use_graph):
-            body(*args)
+            body(*args, host=host)
             return self.prob
         lib = _lib.load()
-        key = args
+        key = args + ("host",) if host else args
         g = self.graphs.get(key)
         if g is None:
             n0 = lib.mivos_launch_count()
-            body(*args)
+            body(*args, host=host)
             self.kernels[key] = lib.mivos_launch_count() - n0
             torch.cuda.current_stream().synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                body(*args)
+                body(*args, host=host)
             lib.mivos_add_launch_count(-self.kernels[key])
             self.graphs[key] = g
             # the eager run above was this tick: a replay would run it twice, and a prefix first appears mid-pass,
@@ -215,34 +233,43 @@ class FrameStep:
             prob_dsts=None, ti: int = 0, graph: bool = True) -> torch.Tensor:
         """`frames[c]` [1,3,nh,nw] (device; read when memorizing) and `cached[c]` the QueryState of clip c's frame;
         `prob_dsts[c]` [(K+1),T,1,nh,nw]: the step writes clip c's result planes to prob_dsts[c][:, ti] itself (None:
-        they are only left in self.prob[c], e.g. for fuse_one_frame).  `graph`: replay the captured graph (the
+        they are only left in self.prob[c], e.g. for fuse_one_frame); a HostResults (host volumes) gets them, with the
+        frame's labels, from one mivos_deliver_planes launch for all such clips.  `graph`: replay the captured graph (the
         calling session's use_graph), else launch eagerly.  Returns self.prob [C,K+1,1,nh,nw]."""
         assert visible <= self.cap_frames and m_front < self.cap_frames
         if visible * self.hw < self.net.min_live_slots:  # same rule as mivos_memory_read and torch.topk
             raise MivosError(f"memory_read: {visible * self.hw} live bank slots < top_k {self.net.top_k}")
-        srcs, dsts = [], []
+        srcs, dsts, recs = [], [], []
         for c in range(self.C):
             q = cached[c]
             srcs += [frames[c].data_ptr() if memorize else 0, q.kv.data_ptr(), q.qk.data_ptr(), q.s8.data_ptr(),
                      q.s4.data_ptr()]
-            dsts += [prob_dsts[c][j, ti].data_ptr() for j in range(self.K + 1)] if prob_dsts is not None else [0] * (self.K + 1)
-        ops.store_words(self.dynp, srcs + dsts, self.dyn, (visible * self.hw, m_front))
+            d = prob_dsts[c] if prob_dsts is not None else None
+            if isinstance(d, HostResults):
+                recs += d.record(ti, c * (self.K + 1))
+                d = None
+            else:
+                recs += [0] * ops.DELIVER_WORDS
+            dsts += [d[j, ti].data_ptr() for j in range(self.K + 1)] if d is not None else [0] * (self.K + 1)
+        host = any(recs)
+        ops.store_words(self.dynp, srcs + dsts + (recs if host else []), self.dyn, (visible * self.hw, m_front))
         if not (graph and self.use_graph):
-            self._body(memorize)
+            self._body(memorize, host)
             return self.prob
         lib = _lib.load()
-        g = self.graphs.get(memorize)
+        key = (memorize, "host") if host else memorize
+        g = self.graphs.get(key)
         if g is None:
             # first use: run eagerly once (allocates every workspace, sets kernel attributes), then capture
             n0 = lib.mivos_launch_count()
-            self._body(memorize)
-            self.kernels[memorize] = lib.mivos_launch_count() - n0
+            self._body(memorize, host)
+            self.kernels[key] = lib.mivos_launch_count() - n0
             torch.cuda.current_stream().synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._body(memorize)
-            lib.mivos_add_launch_count(-self.kernels[memorize])  # capture issued no work
-            self.graphs[memorize] = g
+                self._body(memorize, host)
+            lib.mivos_add_launch_count(-self.kernels[key])  # capture issued no work
+            self.graphs[key] = g
         g.replay()
-        lib.mivos_add_launch_count(self.kernels[memorize])
+        lib.mivos_add_launch_count(self.kernels[key])
         return self.prob

@@ -25,13 +25,21 @@ import torch
 import os
 
 from . import _lib, ops, schedule
+from ._lib import MivosError
 from .engine import QueryState, object_chunks
 from .frame_step import FrameStep
+from .host_results import HostResults
 from .tensor_util import pad_divide_by
 
 
 class InferenceCore:
-    def __init__(self, prop_net, fuse_net, images, num_objects, mem_profile=0, mem_freq=5, device="cuda:0"):
+    def __init__(self, prop_net, fuse_net, images, num_objects, mem_profile=0, mem_freq=5, device="cuda:0",
+                 result_dev=None):
+        """`result_dev`: None keeps prob / masks on the device, for every mem_profile; "cpu" keeps them in
+        page-locked host memory (host_results.HostResults), as the reference's result_dev = 'cpu' does: the
+        device footprint then does not grow with the clip's length, and the results are the same bits."""
+        if result_dev is not None and str(result_dev) != "cpu":  # "cpu" or torch.device("cpu")
+            raise MivosError(f"InferenceCore: result_dev must be None or 'cpu', got {result_dev!r}")
         self.device = torch.device(device)
         _lib.require_cuda_device(self.device, "mivos_b200.InferenceCore")
         self.prop_net = prop_net.to(self.device, non_blocking=True)
@@ -40,8 +48,8 @@ class InferenceCore:
         self.mem_profile = mem_profile
         self.mem_freq = mem_freq
 
-        # Same buffer policy table as the reference (:44-63).  Results always live on the device
-        # here (a 480p prob volume is 1.66 MB per frame per object); the
+        # Same buffer policy table as the reference (:44-63), except for result_dev: results live on the device
+        # unless the caller asks for host results (a 480p prob volume is 1.66 MB per frame per object); the
         # query-feature cache honours q_buf_size, image staging honours data_dev / i_buf_size.
         if mem_profile == 0:
             self.data_dev, self.q_buf_size, self.i_buf_size = self.device, 105, -1
@@ -51,7 +59,7 @@ class InferenceCore:
             self.data_dev, self.q_buf_size, self.i_buf_size = torch.device("cpu"), 3, 3
         else:
             self.data_dev, self.q_buf_size, self.i_buf_size = torch.device("cpu"), 1, 1
-        self.result_dev = self.device
+        self.result_dev = self.device if result_dev is None else torch.device("cpu")
 
         t = images.shape[1]
         h, w = images.shape[-2:]
@@ -67,14 +75,19 @@ class InferenceCore:
         else:
             self.images = self.images.to(self.device).contiguous()
 
-        self.masks = torch.zeros((t, 1, nh, nw), dtype=torch.uint8, device=self.result_dev)  # :77
-        # result masks cross PCIe into ONE pinned staging buffer (async D2H at link rate instead of a
-        # pageable copy); interact() hands the caller a fresh array copied from it, as the reference's
-        # `.cpu().numpy()` does (:269)
-        self._masks_host = torch.zeros((t, h, w), dtype=torch.uint8).pin_memory()
         self.np_masks = np.zeros((t, h, w), dtype=np.uint8)
-        self.prob = torch.zeros((self.k + 1, t, 1, nh, nw), dtype=torch.float32, device=self.result_dev)  # :81
-        self.prob[0] = 1e-7  # :82
+        # host results: prob, masks (:77-82) and the label maps the deliveries keep in page-locked host volumes
+        self._host = None if result_dev is None else HostResults(self.k + 1, t, nh, nw, h, w, self.pad, self.device)
+        if self._host is None:
+            self.masks = torch.zeros((t, 1, nh, nw), dtype=torch.uint8, device=self.result_dev)  # :77
+            # result masks cross PCIe into ONE pinned staging buffer (async D2H at link rate instead of a
+            # pageable copy); interact() hands the caller a fresh array copied from it, as the reference's
+            # `.cpu().numpy()` does (:269)
+            self._masks_host = torch.zeros((t, h, w), dtype=torch.uint8).pin_memory()
+            self.prob = torch.zeros((self.k + 1, t, 1, nh, nw), dtype=torch.float32, device=self.result_dev)  # :81
+            self.prob[0] = 1e-7  # :82
+        else:
+            self.masks, self.prob, self._masks_host = self._host.masks, self._host.prob, None
 
         self.t, self.h, self.w = t, h, w
         self.nh, self.nw = nh, nw
@@ -110,7 +123,7 @@ class InferenceCore:
         self.certain_mem_v = None
         self._certain_bank_k = None  # BANK layout [K, n*hw16, 128]
         self._certain_bank_v = None
-        self._masks_unpadded = torch.zeros((t, h, w), dtype=torch.uint8, device=self.device)
+        self._masks_unpadded = None if self._host else torch.zeros((t, h, w), dtype=torch.uint8, device=self.device)
         self._fuse_planes = None
         self.bank_trace = []  # (frame, visible bank frames) per propagated frame, for plumbing tests
         # CUDA-graph replay of the per-frame step (MIVOS_GRAPH=0: the step's launches are issued eagerly)
@@ -266,6 +279,22 @@ class InferenceCore:
                                                 nc, nr, prob[k - 1, 0])
         return ops.aggregate_any(prob, keep_bg=True)
 
+    # ------------------------------------------------------------------ result frames
+    def _results(self):
+        """Where a frame step delivers this clip's result planes: its prob volume or its host volumes."""
+        return self.prob if self._host is None else self._host
+
+    def _frame(self, ti):
+        """prob[:, ti] on the device."""
+        return self.prob[:, ti] if self._host is None else self._host.load(ti)
+
+    def _set_frame(self, ti, planes):
+        """prob[:, ti] = planes [(K+1),1,nh,nw] (device); host results get the frame's labels with them."""
+        if self._host is None:
+            self.prob[:, ti] = planes
+        else:
+            self._host.store(planes, ti)
+
     # ------------------------------------------------------------------ interaction (:219-271)
     def interact(self, mask, idx, total_cb=None, step_cb=None):
         key_bank_k, key_v = self._begin_interaction(mask, idx, total_cb)
@@ -300,7 +329,7 @@ class InferenceCore:
         self.mask_diff = mask - self.prob[:, idx].to(self.device)  # uses the pre-interaction prob (:233)
         self.pos_mask_diff = self.mask_diff.clamp(0, 1)
         self.neg_mask_diff = (-self.mask_diff).clamp(0, 1)
-        self.prob[:, idx] = mask
+        self._set_frame(idx, mask)
 
         K, hw = self.k, self.hw16
         key_bank_k = torch.empty((K, hw, 128), dtype=torch.float32, device=self.device)
@@ -328,7 +357,14 @@ class InferenceCore:
 
     def _finish_interaction(self):
         """inference_core.py:255-271: argmax over objects for every frame + unpad + u8 as one kernel, one
-        asynchronous D2H into the pinned staging buffer, a fresh array for the caller."""
+        asynchronous D2H into the pinned staging buffer, a fresh array for the caller.  Host results: the
+        deliveries have kept the label maps at argmax(prob) of every frame, so after one synchronisation masks and
+        the returned array are host copies of them."""
+        if self._host is not None:
+            torch.cuda.current_stream(self.device).synchronize()
+            self.masks.copy_(self._host.labels)
+            self.np_masks = self._host.labels_unpadded.numpy().copy()
+            return self.np_masks
         ops.argmax_unpad(self.prob, self.pad, self.h, self.w, self.masks, self._masks_unpadded)
         self._masks_host.copy_(self._masks_unpadded, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
@@ -343,10 +379,14 @@ class InferenceCore:
         clip — per session: eval_interactive_davis.py:83.)"""
         cur = torch.cuda.current_stream(self.device)
         cur.wait_stream(self._qstream)  # nothing of the previous session is still in flight on the side stream
-        self.prob.zero_()
-        self.prob[0] = 1e-7  # :82
-        self.masks.zero_()
-        self._masks_unpadded.zero_()
+        if self._host is not None:
+            cur.synchronize()  # no delivery is still writing the host volumes
+            self._host.fill()
+        else:
+            self.prob.zero_()
+            self.prob[0] = 1e-7  # :82
+            self.masks.zero_()
+            self._masks_unpadded.zero_()
         self.np_masks = np.zeros((self.t, self.h, self.w), dtype=np.uint8)
         self._query_pool.extend(self._query_chunks)
         self.query_buf, self._query_chunks, self._query_ready = {}, [], {}
@@ -410,8 +450,8 @@ def _pass_frame(cores, plan, step, fp, keys, idx, traces):
     # the step stages its operands and (unless the frame is fused) writes every clip's prob[:, ti] itself  # :173-179, :194
     frames = [core.get_image_buffered(ti) if fp.memorize else None for core in cores]
     prob = step.run(frames, cached, fp.visible, fp.m_front, fp.memorize,
-                    prob_dsts=None if plan.fuse else [core.prob for core in cores], ti=ti, graph=cores[0].use_graph)
+                    prob_dsts=None if plan.fuse else [core._results() for core in cores], ti=ti, graph=cores[0].use_graph)
     for c, core in enumerate(cores):
         traces[c].append((ti, fp.visible))
         if plan.fuse:  # :190-194
-            core.prob[:, ti] = core.fuse_one_frame(plan.closest_ti, idx, ti, core.prob[:, ti], prob[c], keys[c], cached[c])
+            core._set_frame(ti, core.fuse_one_frame(plan.closest_ti, idx, ti, core._frame(ti), prob[c], keys[c], cached[c]))

@@ -164,7 +164,7 @@ def _run_ragged_pass(cores, keys, idxs, plans, order, step, step_cb):
         cached = [cores[c].get_query_kv_buffered(fp.ti, plans[c].step, plans[c].closest_ti) for c, fp in zip(act, fps)]
         frames = [cores[c].get_image_buffered(fp.ti) if p < n_mem else None for p, (c, fp) in enumerate(zip(act, fps))]
         prob = step.run_ragged(frames, cached, [fp.visible for fp in fps], [fp.m_front for fp in fps], n_mem,
-                               [None if plans[c].fuse else cores[c].prob for c in act], [fp.ti for fp in fps], graph,
+                               [None if plans[c].fuse else cores[c]._results() for c in act], [fp.ti for fp in fps], graph,
                                ks=ks if mixed else None)
         for p, (c, fp) in enumerate(zip(act, fps)):
             core, plan = cores[c], plans[c]
@@ -172,7 +172,7 @@ def _run_ragged_pass(cores, keys, idxs, plans, order, step, step_cb):
             if plan.fuse:  # :190-194
                 # the clip's planes: prob[p] [K+1,...], or its packed range (background, then its objects)
                 planes = prob[first[p] + p:first[p + 1] + p + 1] if mixed else prob[p]
-                core.prob[:, fp.ti] = core.fuse_one_frame(plan.closest_ti, idxs[c], fp.ti, core.prob[:, fp.ti], planes,
-                                                          keys[c], cached[p])
+                core._set_frame(fp.ti, core.fuse_one_frame(plan.closest_ti, idxs[c], fp.ti, core._frame(fp.ti), planes,
+                                                           keys[c], cached[p]))
         if step_cb is not None:
             step_cb()

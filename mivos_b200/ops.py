@@ -91,6 +91,31 @@ def copy_segments(fixed: torch.Tensor, dyn: torch.Tensor, nbytes: torch.Tensor, 
           "mivos_copy_segments")
 
 
+DELIVER_WORDS = 8  # include/mivos_b200.h: MIVOS_DELIVER_WORDS
+
+
+def deliver_planes(planes: torch.Tensor, table: torch.Tensor, clips: int, nh: int, nw: int) -> None:
+    """Clip c < clips: its planes planes[first_c : first_c + K_c + 1] to its (host-mapped) probability volume at frame
+    ti, and their argmax to its padded and unpadded label maps, as record c of the int64 device table `table`
+    (DELIVER_WORDS words per clip, read when the (captured) launch runs) says; a null volume skips the clip."""
+    _req(planes), _req(table, torch.int64)
+    check(_lib.lib().mivos_deliver_planes(_ptr(planes), _ptr(table), int(clips), int(nh), int(nw), _stream()),
+          "mivos_deliver_planes")
+
+
+def host_register(t: torch.Tensor) -> int:
+    """Page-lock the (pageable, contiguous) CPU tensor `t` in place and return the address kernels write it through."""
+    if t.is_cuda or not t.is_contiguous():
+        raise _lib.MivosError("host_register needs a contiguous CPU tensor")
+    dev = C.c_void_p(0)
+    check(_lib.lib().mivos_host_register(_ptr(t), t.numel() * t.element_size(), C.byref(dev)), "mivos_host_register")
+    return int(dev.value)
+
+
+def host_unregister(t: torch.Tensor) -> None:
+    check(_lib.lib().mivos_host_unregister(_ptr(t)), "mivos_host_unregister")
+
+
 def halo_zeros(n: int, h: int, w: int, c: int, device, dtype=torch.float32) -> torch.Tensor:
     """A HALO map; the border stays zero for the lifetime of the buffer."""
     return torch.zeros((n, h + 2, w + 2, c), dtype=dtype, device=device)
