@@ -216,20 +216,22 @@ def memory_read(bank_k, bank_v, slots, qk, top_k, out, *, out_coff=0, halo_hw=No
     if dyn_slots is not None:  # live slot count read on the device; `slots` is then only the capacity
         slots = int(dyn_slots[0])
     qsets = (qk if qk.dim() == 3 else qk[None]) / (128 ** 0.5)
-    res = []
+    res, sel, sco = [], [], []
     for o in range(k):
         q = qsets[o // q_div if q_div > 0 else 0]
         aff = bank_k[o, :slots] @ q.t()                      # [slots, hw]
         vals, idx = torch.topk(aff, top_k, dim=0)
         wgt = torch.softmax(vals, dim=0)                     # [k, hw]
         res.append(torch.einsum("kq,kqc->qc", wgt, bank_v[o, :slots][idx]))  # [hw, 512]
+        sel.append(idx.t().int())
+        sco.append(vals.t())
     r = torch.stack(res)
     if halo_hw is not None:
         h, w = halo_hw
-        out[:k, 1:-1, 1:-1, out_coff:out_coff + 512] = r.reshape(k, h, w, 512)
+        out[:k, 1:-1, 1:-1, out_coff:out_coff + 512] = r.reshape(k, h, w, 512).to(out.dtype)
     else:
-        out[:, :, out_coff:out_coff + 512] = r
-    return out
+        out[:, :, out_coff:out_coff + 512] = r.to(out.dtype)
+    return (out, torch.stack(sel), torch.stack(sco)) if want_topk else out
 
 
 def upsample2x_add(x, up, n, h, w, x_relu=None, skip=None):

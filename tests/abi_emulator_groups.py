@@ -4,6 +4,8 @@ header's contracts on top of tests/abi_emulator.py's operators.  ``install`` mon
 CPU.  Nothing in the product package imports it."""
 from __future__ import annotations
 
+import torch
+
 import abi_emulator as E
 
 
@@ -15,10 +17,9 @@ def _ranges(first):
 def memory_read_groups(bank_k, bank_v, slots, qk, top_k, out, counts, first, *, out_coff=0, halo_hw=None,
                        workspace=None, algo=0, want_topk=False):
     """Object o of group g (first[g] <= o < first[g+1]) reads query set g over the live slots 0 .. counts[g] - 1."""
-    for g, (a, b) in enumerate(_ranges(first)):
-        E.memory_read(bank_k[a:b], bank_v[a:b], slots, qk[g], top_k, out[a:b], out_coff=out_coff, halo_hw=halo_hw,
-                      dyn_slots=counts[g:g + 1])
-    return out
+    sel = [E.memory_read(bank_k[a:b], bank_v[a:b], slots, qk[g], top_k, out[a:b], out_coff=out_coff, halo_hw=halo_hw,
+                         dyn_slots=counts[g:g + 1], want_topk=want_topk) for g, (a, b) in enumerate(_ranges(first))]
+    return (out, torch.cat([r[1] for r in sel]), torch.cat([r[2] for r in sel])) if want_topk else out
 
 
 def bank_write_groups(halo, n, h, w, coff_k, coff_v, bank_k, bank_v, t_max, dyn_t, first):

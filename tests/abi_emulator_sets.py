@@ -4,6 +4,8 @@ mivos_bank_write_sets), written from the header's contracts on top of tests/abi_
 lock-step host loop runs on the CPU.  Nothing in the product package imports it."""
 from __future__ import annotations
 
+import torch
+
 import abi_emulator as E
 
 
@@ -13,10 +15,10 @@ def memory_read_sets(bank_k, bank_v, slots, qk, top_k, out, counts, *, out_coff=
     0 .. counts[s] - 1 of its own bank."""
     k, sets = bank_k.shape[0], qk.shape[0]
     per = k // sets
-    for s in range(sets):
-        E.memory_read(bank_k[s * per:(s + 1) * per], bank_v[s * per:(s + 1) * per], slots, qk[s], top_k,
-                      out[s * per:(s + 1) * per], out_coff=out_coff, halo_hw=halo_hw, dyn_slots=counts[s:s + 1])
-    return out
+    sel = [E.memory_read(bank_k[s * per:(s + 1) * per], bank_v[s * per:(s + 1) * per], slots, qk[s], top_k,
+                         out[s * per:(s + 1) * per], out_coff=out_coff, halo_hw=halo_hw, dyn_slots=counts[s:s + 1],
+                         want_topk=want_topk) for s in range(sets)]
+    return (out, torch.cat([r[1] for r in sel]), torch.cat([r[2] for r in sel])) if want_topk else out
 
 
 def bank_write_sets(halo, k, sets, h, w, coff_k, coff_v, bank_k, bank_v, t_max, dyn_t):

@@ -13,8 +13,10 @@ Checks per launch (DESIGN.md section 6):
      16 fp16 products per MMA instruction) of the element's own magnitude sum — long K over operands that cancel
      (the 9216-long key/value projection) exceeds the first term alone —, plus, for fp16 and round_tf32 outputs, one
      rounding of the result; round_tf32 outputs also have zero low 13 bits;
-  2. every element of out / out_relu outside [interior rows] x [coff, coff + cout) keeps its bits (HALO border,
-     channels past cout, the neighbouring windows of concat maps), over the whole map;
+  2. every byte of the allocations out / out_relu live in, outside [interior rows] x [coff, coff + cout) of the
+     launch's n maps, keeps its value: the HALO border, channels past cout, the neighbouring windows of concat maps,
+     and the maps of the allocation outside the view (the next object chunk of a logits map sliced lg[k0:k0 + n],
+     the clips past a lock-step tick's prefix);
   3. out_relu == relu(out) on the window;
   4. the premises of the zero padding: the operand's HALO border rows are zero in the read window (9 and 4 taps), the
      packed weights are zero past the real K, and the operand is finite everywhere it is read;
@@ -24,7 +26,8 @@ Check 1 compares every interior row, or, above SAMPLE_MACS multiply-adds, a dete
 `Census.record(scenario)` replaces mivos_b200.ops.conv_gemm — every engine launches through engine._cg — so that each
 eager launch is synchronised, snapshotted, run, polled for a kernel error and checked before the session goes on.
 Launches are deduplicated by signature (layer, shape, types, windows, residual / dual output, plan): the first is
-checked, the rest are counted.  Device-agnostic and importable without a GPU: tests/test_conv_census_cpu.py drives
+checked, the rest are counted.  The plan is (BN, S, CTAs): tile width and split-K factor from mivos_conv_plan, CTAs
+per SM from mivos_conv_plan_residency.  Device-agnostic and importable without a GPU: tests/test_conv_census_cpu.py drives
 `check_launch` with emulated kernels (tests/abi_emulator.py) and mutations of them."""
 from __future__ import annotations
 
@@ -99,6 +102,36 @@ def sample_rows(n: int, h: int, w: int, device, seed: int = 0) -> torch.Tensor:
     return torch.unique(r[interior_mask(r, n, h, w)]).to(device)
 
 
+def storage_bytes(t: torch.Tensor) -> torch.Tensor:
+    """The whole allocation `t` lives in (its untyped storage), as a uint8 tensor sharing it."""
+    return torch.empty(0, dtype=torch.uint8, device=t.device).set_(t.untyped_storage())
+
+
+def like(buf: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
+    """A view of the byte buffer `buf` (a copy of t's allocation) with t's type, offset, shape and strides."""
+    return torch.empty(0, dtype=t.dtype, device=buf.device).set_(buf.untyped_storage(), t.storage_offset(), t.size(),
+                                                                  t.stride())
+
+
+def changed_outside(before: torch.Tensor, t: torch.Tensor, windows, what: str, where=None) -> None:
+    """Raise AssertionError if a byte of t's allocation other than windows(t) differs from `before` (the
+    storage_bytes clone taken before the launch).  `windows(x)` lists the written views of a tensor x laid out as t;
+    `where(e)` names the element at offset e of the view."""
+    exp = before.clone()
+    for a, b in zip(windows(like(exp, t)), windows(t)):
+        a.copy_(b)
+    diff = (exp != storage_bytes(t)).nonzero()
+    if not diff.numel():
+        return
+    byte = int(diff[0, 0])
+    e = byte // t.element_size() - t.storage_offset()
+    if 0 <= e < t.numel() and t.is_contiguous():
+        loc = where(e) if where else f"element {e} of the view"
+    else:
+        loc = f"byte {byte} of the allocation, outside the view of {tuple(t.shape)} at element offset {t.storage_offset()}"
+    raise AssertionError(f"{what} written outside its window: {diff.shape[0]} bytes, first at {loc}")
+
+
 @dataclass
 class Launch:
     """One conv launch: its arguments and snapshots (clones) of what it reads and of its outputs before it ran."""
@@ -110,9 +143,9 @@ class Launch:
     w: int
     x: torch.Tensor                   # operand window [in_rows, cin_pad]
     res: Optional[torch.Tensor]       # residual window [rows, cout], stored type
-    out: torch.Tensor                 # whole output map before the launch
+    out: torch.Tensor                 # the allocation `out` lives in before the launch (bytes)
     out_coff: int
-    out_relu: Optional[torch.Tensor]  # whole ReLU copy before the launch
+    out_relu: Optional[torch.Tensor]  # the allocation of the ReLU copy before the launch (bytes)
     out_relu_coff: int
     relu: bool
     rnd: bool                         # round_tf32 in effect (fp32 outputs only)
@@ -142,8 +175,9 @@ def snapshot(x, pc, n, h, w, out, *, in_coff=0, out_coff=0, relu=False, residual
         out_desc += " +res" + _win(residual, res_coff, pc.cout)[3:]
     if out_relu is not None:
         out_desc += " dual" + _win(out_relu, out_relu_coff, pc.cout)[3:]
-    return Launch(layer, pc, n, h, w, xw, res, out.clone(), out_coff, None if out_relu is None else out_relu.clone(),
-                  out_relu_coff, bool(relu), bool(round_tf32) and out.dtype == torch.float32, plan, in_desc, out_desc)
+    return Launch(layer, pc, n, h, w, xw, res, storage_bytes(out).clone(), out_coff,
+                  None if out_relu is None else storage_bytes(out_relu).clone(), out_relu_coff, bool(relu),
+                  bool(round_tf32) and out.dtype == torch.float32, plan, in_desc, out_desc)
 
 
 def reference(L: Launch, rows: torch.Tensor, with_abs: bool = False):
@@ -191,15 +225,9 @@ def _where(L: Launch, row: int) -> str:
 
 
 def _outside_changed(before, after, L: Launch, coff: int, what: str):
-    C = before.shape[-1]
-    diff = _bits(before.reshape(-1, C)) != _bits(after.reshape(-1, C))
-    diff[:L.rows].view(L.n, L.h + 2, L.w + 2, C)[:, 1:-1, 1:-1, coff:coff + L.pc.cout] = False
-    bad = diff.nonzero()
-    if bad.numel():
-        r, c = int(bad[0, 0]), int(bad[0, 1])
-        raise AssertionError(f"{what} written outside its window: {bad.shape[0]} elements, first at "
-                             f"{_where(L, r)} channel {c} ({float(before.reshape(-1, C)[r, c])} -> "
-                             f"{float(after.reshape(-1, C)[r, c])})")
+    C = after.shape[-1]
+    changed_outside(before, after, lambda t: [window(t, L.n, L.h, L.w, coff, L.pc.cout)], what,
+                    lambda e: f"{_where(L, e // C)} channel {e % C}")
 
 
 def window(t: torch.Tensor, n: int, h: int, w: int, coff: int, cout: int) -> torch.Tensor:
@@ -256,20 +284,25 @@ def check_launch(L: Launch, out, out_relu=None, *, max_macs: float = SAMPLE_MACS
         raise AssertionError(f"{tag}: |got - y| exceeds the bound {worst:.3g}x at {_where(L, r)} channel {c}: got "
                              f"{float(got.reshape(-1)[i])!r}, float64 {float(y.reshape(-1)[i])!r}, max|y| "
                              f"{float(y.abs().max()):.4g}; {int((ratio > 1).sum())} elements over")
-    bn, sp = L.plan if L.plan else (0, 0)
+    bn, sp, ctas = L.plan if L.plan else (0, 0, 0)
+    map_bytes = (L.h + 2) * (L.w + 2) * out.shape[-1] * out.element_size()
     return dict(layer=L.layer, nhw=f"{L.n}x{L.h}x{L.w}", taps=pc.taps, cin_pad=pc.cin_pad, cout=pc.cout,
-                inp=L.in_desc, outp=L.out_desc, bn=bn, s=sp, rows=int(rows.numel()), sampled=sampled, ratio=worst,
+                inp=L.in_desc, outp=L.out_desc, bn=bn, s=sp, ctas=ctas, rows=int(rows.numel()), sampled=sampled,
+                ratio=worst, alloc_maps=L.out.numel() // map_bytes,
                 n=L.n, f16=L.x.dtype == torch.float16, out_f16=out.dtype == torch.float16, res=L.res is not None,
                 dual=L.out_relu is not None, out_coff=L.out_coff, mat=L.in_desc.endswith("mat"))
 
 
 def conv_plan(x, pc, n, h, w, out, kw, sms: int = 0):
-    """(BN, S) that mivos_conv_plan reports for the argument block ops.conv_gemm builds from these arguments."""
+    """(BN, S, CTAs per SM) that mivos_conv_plan and mivos_conv_plan_residency report for the argument block
+    ops.conv_gemm builds from these arguments."""
     from mivos_b200 import _lib, ops
     a = ops.conv_args(x, pc, n, h, w, out, **kw)
-    bn, sp = C.c_int(0), C.c_int(0)
-    _lib.check(_lib.load().mivos_conv_plan(C.byref(a), sms, C.byref(bn), C.byref(sp)), "mivos_conv_plan")
-    return bn.value, sp.value
+    bn, sp, ctas = C.c_int(0), C.c_int(0), C.c_int(0)
+    lib = _lib.load()
+    _lib.check(lib.mivos_conv_plan(C.byref(a), sms, C.byref(bn), C.byref(sp)), "mivos_conv_plan")
+    _lib.check(lib.mivos_conv_plan_residency(C.byref(a), sms, C.byref(ctas)), "mivos_conv_plan_residency")
+    return bn.value, sp.value, ctas.value
 
 
 class Census:
@@ -335,11 +368,11 @@ class Census:
 
     def table(self) -> str:
         head = (f"{'scenario':24s} {'layer':44s} {'n x h x w':>13s} {'taps':>4s} {'cin_p':>5s} {'cout':>4s} "
-                f"{'in':24s} {'out':44s} {'BN':>3s} {'S':>2s} {'rows':>8s} {'err/bound':>9s}")
+                f"{'in':24s} {'out':44s} {'BN':>3s} {'S':>2s} {'CTA':>3s} {'rows':>8s} {'err/bound':>9s}")
         lines = [head]
         for r in self.records:
             lines.append(f"{r['scenario']:24s} {r['layer']:44s} {r['nhw']:>13s} {r['taps']:4d} {r['cin_pad']:5d} "
-                         f"{r['cout']:4d} {r['inp']:24s} {r['outp']:44s} {r['bn']:3d} {r['s']:2d} "
+                         f"{r['cout']:4d} {r['inp']:24s} {r['outp']:44s} {r['bn']:3d} {r['s']:2d} {r['ctas']:3d} "
                          f"{r['rows']:8d}{'*' if r['sampled'] else ' '}{r['ratio']:9.3g}")
         return "\n".join(lines)
 

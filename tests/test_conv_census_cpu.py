@@ -278,6 +278,25 @@ def test_check_rejects_mutation(mutation, act, max_macs):
         _run(lambda *a, **k: _emulated(*a, mutate=fn, **k), _case(act, **extra), max_macs)
 
 
+@pytest.mark.parametrize("act", list(DTYPES))
+def test_check_rejects_a_write_into_the_next_chunk(act):
+    """`out` is the chunk view lg[k0:k0 + n] of a logits map of more objects: a kernel that writes one element into
+    the next chunk's first map writes inside the allocation but outside the view, and must fail."""
+    x, pc, n, h, w, out, kw = _case(act, res=False, dual=False)
+    parent = torch.full((2 * n + 2, h + 2, w + 2, out.shape[-1]), -7.0, dtype=out.dtype)
+    chunk = parent[2:2 + n]
+    rec = _run(_emulated, (x, pc, n, h, w, chunk, kw))
+    assert rec["ratio"] <= 1.0 and rec["alloc_maps"] == 2 * n + 2
+
+    def spill(stage, v):
+        if stage == "out":
+            parent[2 + n, 3, 4, 64] = 0.5  # interior element of the window's channels, one map past the view
+        return v
+    parent.fill_(-7.0)
+    with pytest.raises(AssertionError, match="outside the view"):
+        _run(lambda *a, **k: _emulated(*a, mutate=spill, **k), (x, pc, n, h, w, chunk, kw))
+
+
 def test_premise_checks_reject_dirty_operands():
     x, pc, n, h, w, out, kw = _case("tf32")
     x[0, 0, 4, 3] = 1.0  # a HALO border element of the operand
