@@ -18,7 +18,6 @@ Every lane partial takes one rounding per term and one per tile multiply: (5T + 
 the 5 levels of the warp tree.  The map is the W-weighted mean of the pooled masks (an error shared by all terms
 cancels), as for the resident kernel; W's second pass uses the final maximum, so its exponentials carry the resident
 kernel's eps, and only the denominator carries the streamed errors."""
-import math
 
 import pytest
 import torch
@@ -27,100 +26,14 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 from mivos_b200 import _lib, ops  # noqa: E402
-from test_gpu_ops_ragged import (GAMMA, H16, NAN, SENT, U, _check, _check_stem, _stem_out,  # noqa: E402
-                                 stem_images, stem_matrix)
-
-SK = 128  # keys per tile of attention_stream_kernel
-TINY = 2.0 ** -149
-BLOCK = 1024  # query columns per float64 block
+from op_references import SK, map_reference, stem_images, stem_matrix, weights_streamed_blocks  # noqa: E402
+from test_gpu_ops_ragged import H16, NAN, SENT, _check, _check_stem, _stem_out  # noqa: E402
 
 
 def _worst(what, ratios):
     r = max(ratios)
     print(f"{what}: max err/bound = {r:.3g}")
     return r
-
-
-def _tiles(x, fill):
-    """[hw, nb] -> [T, SK, nb] padded with `fill`."""
-    hw, nb = x.shape
-    T = -(-hw // SK)
-    p = torch.full((T * SK, nb), fill, dtype=x.dtype, device=x.device)
-    p[:hw] = x
-    return p.reshape(T, SK, nb)
-
-
-def stream_blocks(mk, qk, pooled=None, row_lse=None):
-    """Yields, per block of query columns [j0, j1): float64 logits and softmax W over the memory axis, the streamed
-    kernel's per-term relative error eps (with rescales) and the resident kernel's eps_r; with pooled also the map,
-    and with row_lse (logsumexp over queries of every memory row) the map of a softmax over the QUERY axis."""
-    hw = mk.shape[0]
-    m, q = mk.double(), qk.double()
-    for j0 in range(0, hw, BLOCK):
-        j1 = min(hw, j0 + BLOCK)
-        L = m @ q[j0:j1].t() / math.sqrt(128)
-        S = m.abs() @ q[j0:j1].abs().t() / math.sqrt(128)
-        Lmax = L.max(0, keepdim=True).values
-        W = torch.softmax(L, 0)
-        G = GAMMA * _tiles(S, 0.0).max(1).values  # [T, nb]: |fp32 tile max - float64 tile max| <= G
-        tmax = _tiles(L, -math.inf).max(1).values
-        lo = torch.cummax(tmax - G, 0).values
-        possible = torch.zeros_like(tmax)
-        possible[1:] = ((tmax[1:] + G[1:]) > lo[:-1]).double()
-        after = possible.flip(0).cumsum(0).flip(0) - possible  # rescales strictly after tile t
-        R = after.repeat_interleave(SK, 0)[:hw]
-        base = GAMMA * (S + S.max(0, keepdim=True).values)
-        dl = (L - Lmax).abs()
-        del S
-        eps = base + 2 * U * dl + 4 * U * (1 + R)
-        eps_r = base + U * dl + 4 * U
-        blk = dict(j0=j0, j1=j1, L=L, W=W, eps=eps, eps_r=eps_r, tmax=tmax)
-        if pooled is not None:
-            blk["map"] = pooled @ W
-        if row_lse is not None:
-            blk["map_qaxis"] = pooled @ torch.exp(L - row_lse[:, None])
-        yield blk
-
-
-def map_reference(mk, qk, h16, w16, pos, neg, mistakes=False):
-    """float64 map [1,2,H,W], the streamed bound, the resident bound (same formula as attention_reference), and with
-    `mistakes` the maps of three kernel mistakes: the last tile skipped, no rescale, the softmax over queries."""
-    hw = h16 * w16
-    T = -(-hw // SK)
-    pooled = torch.cat([F.avg_pool2d(pos.double(), 16), F.avg_pool2d(neg.double(), 16)], 1).reshape(2, hw)
-    row_lse = None
-    if mistakes:
-        m, q = mk.double(), qk.double()
-        row_lse = torch.full((hw,), -math.inf, dtype=torch.float64, device=mk.device)
-        for j0 in range(0, hw, BLOCK):
-            row_lse = torch.logaddexp(row_lse, torch.logsumexp(m @ q[j0:j0 + BLOCK].t() / math.sqrt(128), 1))
-    g_s = (5 * T + 6) * U
-    g_r = (math.ceil(hw / 32) + 6) * U
-    mp = torch.empty(2, hw, dtype=torch.float64, device=mk.device)
-    mb, mbr = torch.empty_like(mp), torch.empty_like(mp)
-    bad = {k: torch.empty_like(mp) for k in ("skip_last_tile", "no_rescale", "query_axis")} if mistakes else {}
-    for b in stream_blocks(mk, qk, pooled, row_lse):
-        j0, j1, W, mapb = b["j0"], b["j1"], b["W"], b["map"]
-        mp[:, j0:j1] = mapb
-        for k in range(2):
-            dev_ = (pooled[k][:, None] - mapb[k][None, :]).abs()
-            mb[k, j0:j1] = (W * b["eps"] * dev_).sum(0)
-            mbr[k, j0:j1] = (W * b["eps_r"] * dev_).sum(0)
-        if mistakes:
-            L = b["L"]
-            cut = (T - 1) * SK
-            bad["skip_last_tile"][:, j0:j1] = pooled[:, :cut] @ torch.softmax(L[:cut], 0)
-            run = torch.cummax(b["tmax"], 0).values.repeat_interleave(SK, 0)[:hw]  # running max after each key's tile
-            e = torch.exp(L - run)
-            bad["no_rescale"][:, j0:j1] = (pooled @ e) / e.sum(0)
-            bad["query_axis"][:, j0:j1] = b["map_qaxis"]
-    mb = mb + mp * (255 * U + 2 * g_s + U) + 2 * hw * TINY
-    mbr = mbr + mp * (255 * U + 2 * g_r + U)
-    H, Wd = 16 * h16, 16 * w16
-    up = lambda x: F.interpolate(x.reshape(1, 2, h16, w16), size=(H, Wd), mode="bilinear", align_corners=False)  # noqa: E731
-    out = up(mp)
-    lift = 4 * U * up(mp.abs())
-    return out, up(mb) + lift, up(mbr) + lift, {k: up(v) for k, v in bad.items()}
 
 
 def _inputs(h16, w16, scale, seed, dev):
@@ -198,14 +111,8 @@ def test_attention_weights_streamed(dev, hw, scale):
     _lib.poll_kernel_error()
     assert bool((out[hw * hw:] == SENT).all()), "wrote past W"
     Wg = out[:hw * hw].view(hw, hw)
-    T = -(-hw // SK)
-    g_s = (5 * T + 6) * U
     ratios = []
-    blocks = list(stream_blocks(mk, qk))
-    for b in blocks:
-        j0, j1, W = b["j0"], b["j1"], b["W"]
-        d_den = (W * b["eps"]).sum(0, keepdim=True) + g_s + hw * TINY
-        Wb = W * (b["eps_r"] + d_den + U) + 4 * TINY
+    for j0, j1, W, Wb in weights_streamed_blocks(mk, qk):
         err = (Wg[:, j0:j1].double() - W).abs()
         ratios.append(float((err / Wb).max()))
     r = _worst(f"attention_weights_streamed hw={hw} x{scale:g}", ratios)

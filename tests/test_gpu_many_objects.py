@@ -14,8 +14,9 @@ from mivos_b200 import _lib, ops  # noqa: E402
 from mivos_b200.engine import object_chunks  # noqa: E402
 from oracle import gen_golden_objects as GO  # noqa: E402  (input recipes of the goldens)
 from oracle import weights as Wt  # noqa: E402  (synthetic clips only)
-from test_gpu_ops_ragged import (NAN, SENT, U, _bilinear, _check, _halo, _logits, _sum_and_range,  # noqa: E402
-                                 aggregate_reference)
+from op_references import (U, _bilinear, _sum_and_range, aggregate_reference, stem_reference,  # noqa: E402,F401
+                           stem_tolerance)
+from test_gpu_ops_ragged import NAN, SENT, _check, _halo, _logits  # noqa: E402
 
 P_MAX, P_MEAN = 3e-2, 1e-3
 SHAPES = ((1, 1), (3, 5), (7, 9))  # (h4, w4): ragged pixel counts, 16 to 1008 pixels per plane
@@ -116,25 +117,6 @@ def test_drop_in_aggregate_takes_255_objects(dev, golden):
 
 
 # ------------------------------------------------------------------------------------------------ stem gather
-def stem_reference(frame, masks, k0, n):
-    """float64 space-to-depth memorize stem of objects [k0, k0 + n): channels (frame, own mask, sum of every OTHER
-    mask of the K); out[row(Y,X), py*40 + j*5 + c] = in[c, 2Y+py, 2X-4+j]."""
-    import abi_emulator
-    f, m = frame.double().cpu(), masks.double().cpu()
-    total = m.sum(0)
-    inp = torch.cat([f.expand(n, -1, -1, -1), m[k0:k0 + n], total[None].expand(n, -1, -1, -1) - m[k0:k0 + n]], 1)
-    H, W = f.shape[-2:]
-    out = torch.zeros((n * (H // 2 + 2) * (W // 2 + 2), 80), dtype=torch.float64)
-    abi_emulator._stem_s2d_frames(inp, out)
-    return out
-
-
-def stem_tolerance(ref, K, f16):
-    """fp32 sequential sum of K - 1 masks in [0, 1]: (K - 1) u of the sum; fp16 storage adds one rounding (and half
-    of its smallest subnormal step below 2^-14)."""
-    return ref.abs() * ((K - 1) * U + (2.0 ** -11 if f16 else 0.0)) + (2.0 ** -24 if f16 else 0.0)
-
-
 @pytest.mark.parametrize("f16", [False, True])
 def test_stem_gather_range(dev, f16):
     dt = torch.float16 if f16 else torch.float32

@@ -12,7 +12,6 @@ slots.  Inputs a kernel must not read (HALO borders of bilinear sources, channel
 a sentinel, so a stray read shows up in the output."""
 import math
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -20,9 +19,10 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 from mivos_b200 import _lib, ops  # noqa: E402
+from op_references import (CLAMP_HI, CLAMP_LO, GAMMA, H16, U, _bilinear, _sum_and_range,  # noqa: E402,F401
+                           aggregate_reference, attention_reference, stem_images, stem_matrix)
+from op_references import round16 as _round16  # noqa: E402
 
-U = 2.0 ** -24  # unit roundoff of fp32 (round to nearest)
-H16 = torch.float16
 VEC = {torch.float32: 4, torch.float16: 8}  # elements per 16-byte vector
 SENT = 7.0
 NAN = float("nan")
@@ -46,56 +46,7 @@ def _halo(x, cstride, coff=0, fill=0.0, border=None, dtype=torch.float32):
     return hb
 
 
-def _bilinear(x, h, w):
-    """fp64 bilinear resize, align_corners=False (the kernels' source-index convention)."""
-    return F.interpolate(x.double(), size=(h, w), mode="bilinear", align_corners=False)
-
-
 # ------------------------------------------------------------------------------------------------ attention
-# Logit s_ij = sum_c mk_ic * fl(qk_jc / fl(sqrt 128)): the fp32 constant and the division round once each, the
-# 128-term fma chain rounds 128 times, so |s_ij - L_ij| <= GAMMA * S_ij with S_ij = sum_c |mk_ic qk_jc| / sqrt(128).
-GAMMA = 130 * U
-
-
-def attention_reference(mk, qk, h16=None, w16=None, pos=None, neg=None):
-    """fp64 W[i, j] = softmax_i(mk_i . qk_j / sqrt(128)) with its elementwise bound; with pos/neg also the map
-    bilinear_x16(area16(pos|neg) @ W) and its bound."""
-    hw = mk.shape[0]
-    m, q = mk.double(), qk.double()
-    L = m @ q.t() / math.sqrt(128)  # [memory i, query j]
-    S = m.abs() @ q.abs().t() / math.sqrt(128)
-    Lmax = L.max(0, keepdim=True).values
-    W = torch.softmax(L, 0)
-    # relative error of e_ij = expf(fl(s_ij - m_j)): the logit and the column max (|m_j - Lmax_j| <= GAMMA max_i S_ij),
-    # one rounding of the difference (u |L_ij - Lmax_j|), 2 ulp of expf (4u)
-    eps = GAMMA * (S + S.max(0, keepdim=True).values) + U * (L - Lmax).abs() + 4 * U
-    del S
-    # den_j = sum_i e_ij: ceil(hw/32) additions per lane + 5 levels of the warp tree, +1 for gamma_n ~ n u
-    g_den = (math.ceil(hw / 32) + 6) * U
-    d_den = (W * eps).sum(0, keepdim=True) + g_den  # relative error of den_j: the e_ij errors weighted by W_ij
-    # W_ij = fl(e_ij / den_j): + one rounding; expf and the quotient lose relative precision below 2^-126, where
-    # their absolute error stays within 4 * 2^-149
-    Wb = W * (eps + d_den + U) + 4 * 2.0 ** -149
-    if pos is None:
-        return W, Wb
-    pooled = torch.cat([F.avg_pool2d(pos.double(), 16), F.avg_pool2d(neg.double(), 16)], 1).reshape(2, hw)
-    mp = pooled @ W  # [2, hw]
-    # map_j = pp_j / den_j is the W-weighted mean of pooled, so to first order the e_ij errors enter only as
-    # sum_i W_ij eps_ij |pooled_i - map_j| (an error common to all e_ij cancels).  pooled_i >= 0 is 255 sequential
-    # fp32 additions (the /256 is exact): 255u of it, i.e. 255u map_j after weighting; pp_j and den_j round g_den
-    # each; the quotient rounds once
-    We = W * eps
-    del eps
-    mb = torch.stack([(We * (pooled[k][:, None] - mp[k][None, :]).abs()).sum(0) for k in range(2)])
-    mb = mb + mp * (255 * U + 2 * g_den + U)
-    del We
-    H, Wd = 16 * h16, 16 * w16
-    out = _bilinear(mp.reshape(1, 2, h16, w16), H, Wd)
-    # x16 bilinear: exact weights (multiples of 1/32), at most 4 roundings on each corner term, and nonnegative
-    # weights carry the map bound through
-    outb = _bilinear(mb.reshape(1, 2, h16, w16), H, Wd) + 4 * U * _bilinear(mp.abs().reshape(1, 2, h16, w16), H, Wd)
-    return W, Wb, out, outb
-
 
 def _attention_inputs(h16, w16, scale, seed, dev):
     g = torch.Generator().manual_seed(seed)
@@ -171,42 +122,6 @@ def test_attention_rejections(dev):
 
 
 # ------------------------------------------------------------------------------------------------ aggregation
-CLAMP_LO = float(np.float32(1e-7))  # the kernel's fp32 clamp bounds, not the decimal constants
-CLAMP_HI = float(np.float32(1.0) - np.float32(1e-7))
-assert CLAMP_HI == 1.0 - 2.0 ** -23
-
-
-def aggregate_reference(p, const_bg=False):
-    """fp64 aggregate_wbg of the fp32 object probabilities p [K, ...] (the kernel's operands, exactly):
-    softmax over [bg, p_1..p_K] of logit(clamp(.)), with bg = prod(1 - p) (0.5 for const_bg); and its bound."""
-    K = p.shape[0]
-    v = p.double()
-    bg = torch.full_like(v[:1], 0.5) if const_bg else torch.prod(1 - v, 0, keepdim=True)
-    x = torch.cat([bg, v], 0).clamp(CLAMP_LO, CLAMP_HI)
-    lg = torch.log(x / (1 - x))
-    o = torch.softmax(lg, 0)
-    # relative error of the fp32 operand: bg is K roundings of 1 - p_j and K - 1 of the product; p_j are exact
-    rho = torch.zeros_like(x)
-    if not const_bg:
-        rho[0] = 2 * K * U
-    # absolute error of each fp32 logit: the operand's error through d logit / dx = 1 / (x (1 - x)), one rounding
-    # each for 1 - x and the quotient, 1 ulp of logf (<= 2u |logit|)
-    eta = rho / (1 - x) + 2 * U + 2 * U * lg.abs()
-    # relative error of e_j = expf(fl(l_j - max)): eta_j, the rounded difference, 2 ulp of expf.  o_j = e_j / s:
-    # s carries the e errors weighted by o plus K additions, and the quotient rounds once
-    a = eta + U * (lg - lg.max(0, keepdim=True).values).abs() + 4 * U
-    bound = o * (a + (o * a).sum(0, keepdim=True) + (K + 1) * U)
-    return o, bound, lg
-
-
-def _sum_and_range(what, o, K):
-    """Every pixel of [bg, objects] sums to 1 within (K+1) 2^-23 (K additions in the denominator and one rounding
-    per quotient: (K+1) 2^-24 to first order, doubled for the higher-order terms), every value in [0, 1]."""
-    s = o.double().sum(0)
-    ratio = float(((s - 1).abs() / ((K + 1) * 2.0 ** -23)).max())
-    print(f"{what}: max |sum - 1| / bound = {ratio:.3g}")
-    assert ratio <= 1.0, f"{what}: max |sum - 1| / bound = {ratio:.3g}"
-    assert bool(((o >= 0) & (o <= 1)).all()), what
 
 
 def _logits(groups, K, h4, w4, seed):
@@ -521,47 +436,6 @@ def test_halo_sigmoid_to_plane_ragged(dev):
 
 
 # ------------------------------------------------------------------------------------------------ stem gathers
-def stem_images(frames, masks=None):
-    """fp64 input images of a stem gather [N, cin, H, W] and the bound of each value.  frames alone: a batch of
-    3- or 6-channel images.  frames [G, 3, H, W] with masks [G, K, H, W]: per object (group-major) the frame, its own
-    mask and the exact sum of the other objects' masks.  The kernel adds the K - 1 other masks to 0 in object order,
-    the first addition exact: |others - sum| <= (K - 2) u sum_{j != k} m_j.  Every other channel is one rounding of
-    the fp32 operand to the map type, applied by the caller."""
-    if masks is None:
-        img = frames.double()
-        return img, torch.zeros_like(img)
-    G, K = masks.shape[:2]
-    m = masks.double()
-    imgs, bounds = [], []
-    for k in range(K):
-        others = torch.cat([m[:, :k], m[:, k + 1:]], 1).sum(1, keepdim=True)
-        imgs.append(torch.cat([frames.double(), m[:, k:k + 1], others], 1))
-        b = torch.zeros_like(imgs[-1])
-        b[:, 4:] = max(K - 2, 0) * U * others
-        bounds.append(b)
-    N = G * K
-    return torch.stack(imgs, 1).reshape(N, 5, *frames.shape[2:]), torch.stack(bounds, 1).reshape(N, 5, *frames.shape[2:])
-
-
-def stem_matrix(img, kpad, s2d):
-    """The gather of img [N, cin, H, W] as the kernels write it: HALO rows of the half-resolution output map, kpad
-    columns.  49 taps: the F.unfold(7, stride 2, pad 3) windows in (ky, kx, c) order.  s2d (header formula):
-    out[row(Y, X), py*8*cin + j*cin + c] = in[c, 2Y + py, 2X - 4 + j], zero outside the image.  Border rows and the
-    pad columns are zero."""
-    N, cin, H, W = img.shape
-    ho, wo = H // 2, W // 2
-    if s2d:
-        p = F.pad(img, (4, 4))
-        cols = torch.stack([p[:, :, py::2, j:j + 2 * wo:2] for py in range(2) for j in range(8)], 1)  # [N, 16, cin, ho, wo]
-        cols = cols.permute(0, 3, 4, 1, 2).reshape(N, ho, wo, 16 * cin)
-    else:
-        cols = F.unfold(img, 7, padding=3, stride=2).reshape(N, cin, 49, ho, wo).permute(0, 3, 4, 2, 1)
-        cols = cols.reshape(N, ho, wo, 49 * cin)
-    out = torch.zeros((N, ho + 2, wo + 2, kpad), dtype=torch.float64, device=img.device)
-    out[:, 1:-1, 1:-1, :cols.shape[-1]] = cols
-    return out.reshape(-1, kpad)
-
-
 def _stem_out(N, H, W, kpad, dtype, dev):
     """A matrix of N * (H/2 + 2) * (W/2 + 2) rows filled with the sentinel, plus one guard row past its end."""
     rows = N * (H // 2 + 2) * (W // 2 + 2)
@@ -590,13 +464,6 @@ def _check_stem(what, buf, img, bound, kpad, s2d, dtype):
     live = (ro != 0) | (bo != 0)
     assert torch.equal(go[~live], ro[~live]), f"{what}: others in the zero padding"
     _check(f"{what} others", go[live], ro[live], bo[live])
-
-
-def _round16(bound, ref, dtype):
-    """A bound on an fp32 value, widened by its final rounding to an fp16 map (2^-25 absolute below the normal range)."""
-    if dtype != H16:
-        return bound
-    return bound * (1 + 2.0 ** -11) + 2.0 ** -11 * ref.abs() + 2.0 ** -25
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, H16])

@@ -26,6 +26,7 @@ pytestmark = pytest.mark.gpu
 
 from mivos_b200 import _lib, ops  # noqa: E402
 from test_gpu_ops_ragged import H16, NAN, SENT, U, VEC, _check, _halo, _round16  # noqa: E402
+from op_references import avgpool_reference, bilinear_reference  # noqa: E402
 
 DT = {"fp16": torch.float16, "tf32": torch.float32}
 
@@ -76,16 +77,6 @@ def test_gather_dilated(dev, dtype, dil):
 
 
 # ------------------------------------------------------------------------------------------ pooled broadcast
-def avgpool_reference(x):
-    """fp64 mean over the pixels of x [n, c, h, w] and its bound for the kernel's summation order (module docstring)."""
-    n, c, h, w = x.shape
-    hw = h * w
-    xd = x.double()
-    mu = xd.mean((2, 3))
-    s = xd.abs().sum((2, 3))
-    return mu, (math.ceil(hw / 8) + 7) * U * s / hw + 2 * U * mu.abs()
-
-
 # (n, h, w, c, in_coff, out_coff, spread of the per-image offsets, common offset)
 AVGPOOL_CASES = [
     (2, 1, 1, None, 0, 0, 0.0, 0.0),      # hw = 1
@@ -119,22 +110,6 @@ def test_avgpool_broadcast(dev, dtype, case):
 
 
 # ------------------------------------------------------------------------------------------ bilinear resizes
-def bilinear_reference(x, h, w):
-    """fp64 F.interpolate(size=(h, w), align_corners=False) of x [n, c, hs, ws] and the kernels' bound on it
-    (module docstring)."""
-    hs, ws = x.shape[-2:]
-    xd = x.double()
-    ref = F.interpolate(xd, size=(h, w), mode="bilinear", align_corners=False)
-    mag = F.interpolate(xd.abs(), size=(h, w), mode="bilinear", align_corners=False)
-    exact = all(math.log2(a / b).is_integer() for a, b in ((hs, h), (ws, w)))
-    bound = (5 if exact else 6) * U * mag
-    if not exact:
-        dy = float(xd.diff(dim=2).abs().max()) if hs > 1 else 0.0
-        dx = float(xd.diff(dim=3).abs().max()) if ws > 1 else 0.0
-        bound = bound + 3 * U * (hs + 1) * dy + 3 * U * (ws + 1) * dx
-    return ref, bound
-
-
 # (n, hs, ws, h, w, c (None: a ragged count), src_coff, dst_coff)
 RESIZE_CASES = [
     (1, 45, 80, 180, 320, 256, 1, 48),  # x4, the S2M head at 720p: ASPP output into the 304-channel concat map
