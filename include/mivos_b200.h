@@ -303,7 +303,9 @@ MIVOS_API int mivos_memory_read_wide(const float* bank_k, const float* bank_v, i
  * clamped to slots_cap.  Slots at or past a set's count take no part in that set's read (they may hold stale data
  * or NaN).  Everything else — operands, output window, workspace sizes, topk_idx / topk_val, algo — is that of the
  * scalar form; with every count equal to n a per-set read gives the bits of the scalar read with dyn_slots = n and
- * q_div = k_objects / sets.                                                                                        */
+ * q_div = k_objects / sets.  A count below top_k (`slots` bounds no count) selects every live slot: topk_idx is padded
+ * with -1 and topk_val with 0 past them, the read-out is the softmax over the live slots, and a count of 0 writes
+ * zeros; the top-k and wide reads give the same bits there as well (top_k <= 64).                                  */
 MIVOS_API int mivos_memory_read_sets(const float* bank_k, const float* bank_v, int64_t slots_cap,
                       int k_objects, int64_t slots, const float* qk, int hw, int sets, int top_k,
                       void* out, int out_cstride, int out_coff, int out_halo_h, int out_halo_w,
